@@ -577,7 +577,8 @@ struct BodyArgs {
   uint64_t n_groups;
   uint32_t* hits;              // in: alive masks (when has_alive), out: final hit masks
   int has_alive;
-  unsigned long long* counter; // [1] = tile bytes of the groups entered, [3] = tile bytes requested, [4] = live records (gather)
+  unsigned long long* counter; // [1] = tile bytes of the groups entered, [3] = tile bytes requested (k_body: 16 per lane and
+                               // row it loaded), [4] = live records (gather)
   unsigned long long gather_max;   // k_body_sticky stands down (and k_body_gather runs) when 0 < counter[4] <= gather_max
   // one launch covers the groups [g_begin, n_groups): the scan is cut into chunks of whole windows so that the compaction
   // (and, multi-GPU, the all-gather) of a finished chunk overlaps the next chunk's scan; *next hands out the chunk's groups
@@ -688,13 +689,61 @@ struct BodyDfa {
   }
 };
 
+// Early exit of k_body (kAcc 0 / 1 / 2).  A record's content verdict acc = OR of out[] over the states it visits | endout[final
+// state] only ever gains bits, and its hit mask reads no bit of acc but those of the body conditions of its alive queries
+// (`need`).  Once every bit of `need` is set by the out[] of a visited state, each of those conditions is decided whatever the
+// rest of the record holds (a negated one is false for good), so a lane that stops there writes the hit mask the full scan
+// would: finish() sets the same bits of `need`, and the other bits of acc are not read.  Bits that only endout[] sets ($, \Z)
+// never enter the running mask, so records that need them are read to the end.
+// The check runs between blocks of kDecideRows rows, outside the row loop: a check inside it, even one every 4th row, made
+// every row slower on H100 than the skipped lookups saved (DESIGN 5.1).  The
+// accepting states visited since the last check are folded into `rem` (the bits of need still unset), each at most once per
+// record (`folded`).
+constexpr uint32_t kDecideRows = 16;
+template <int kAcc>
+struct BodyDecide {
+  using Bits = typename std::conditional<kAcc == 2, unsigned long long, uint32_t>::type;
+  uint32_t rem;                // bits of need not yet set
+  Bits folded;                 // accepting states already folded into rem (and the bit positions of non-accepting states)
+  __device__ __forceinline__ void reset(uint32_t need, uint32_t n_acc) {
+    rem = need;
+    if (kAcc == 1) folded = n_acc >= 32 ? 0u : ~0u << n_acc;
+    if (kAcc == 2) folded = n_acc >= 64 ? 0ull : ~0ull << n_acc;
+  }
+  template <bool kDirect>
+  __device__ __forceinline__ bool decided(const BodyDfa<kDirect, kAcc>& d) {
+    if (kAcc == 0) rem &= ~d.a0;                              // a0 holds the pattern masks already
+    if (kAcc == 1 || kAcc == 2) {
+      Bits fresh = (kAcc == 1 ? (Bits)d.a0 : (Bits)d.a64) & ~folded;
+      if (fresh) {
+        folded |= fresh;
+        do { rem &= ~d.out[__ffsll((long long)fresh) - 1]; fresh &= fresh - 1; } while (fresh);
+      }
+    }
+    return rem == 0;
+  }
+};
+
 template <bool kDirect, int kAcc, bool kPush>
 __global__ void __launch_bounds__(kBodyThreads, 1) k_body(BodyArgs a) {
   extern __shared__ __align__(128) uint8_t smem[];
   __shared__ uint64_t bar;
+  __shared__ uint32_t q_need[33];                  // [q] = content bits the conditions of query q read; [32] = OR over all queries
   const fei_prog_hdr* ph = reinterpret_cast<const fei_prog_hdr*>(a.prog);
   const fei_prog_dfa* dd = reinterpret_cast<const fei_prog_dfa*>(a.prog + ph->off_body_dfa);
   const uint32_t table_bytes = dd->table_bytes;
+  const fei_prog_cond* conds = reinterpret_cast<const fei_prog_cond*>(a.prog + ph->off_conds);
+  const fei_prog_query* queries = reinterpret_cast<const fei_prog_query*>(a.prog + ph->off_queries);
+  const uint32_t nq = ph->n_queries;
+  if (kAcc != 3 && threadIdx.x < 32) {
+    uint32_t bits = 0;
+    if (threadIdx.x < nq)
+      for (uint32_t c = queries[threadIdx.x].cond_begin; c < queries[threadIdx.x].cond_end; ++c)
+        if (conds[c].kind == FEI_C_BODY) bits |= 1u << conds[c].bit;
+    q_need[threadIdx.x] = bits;
+    bits = __reduce_or_sync(0xffffffffu, bits);
+    if (threadIdx.x == 0) q_need[32] = bits;
+  }
   // ---- stage the automaton into shared memory with TMA bulk copies (cp.async.bulk + mbarrier)
   if (threadIdx.x == 0) { mbar_init(&bar, 1); asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
   __syncthreads();
@@ -709,13 +758,12 @@ __global__ void __launch_bounds__(kBodyThreads, 1) k_body(BodyArgs a) {
   mbar_wait(&bar, 0);
   const uint32_t* endout = reinterpret_cast<const uint32_t*>(smem + (dd->off_endout - dd->off_trans));
   const uint32_t start = dd->start;
-  const fei_prog_cond* conds = reinterpret_cast<const fei_prog_cond*>(a.prog + ph->off_conds);
-  const fei_prog_query* queries = reinterpret_cast<const fei_prog_query*>(a.prog + ph->off_queries);
-  const uint32_t nq = ph->n_queries;
   const uint32_t all_q = nq >= 32 ? 0xFFFFFFFFu : ((1u << nq) - 1u);
   const int lane = threadIdx.x & 31;
-  unsigned long long touched = 0, bytes_read = 0;
+  unsigned long long touched = 0;
+  uint32_t rows_read = 0;                          // rows of 16 bytes this lane requested
   BodyDfa<kDirect, kAcc> d;
+  BodyDecide<kAcc> dec;
   d.trans_s = smem_u32(smem);
   d.out = reinterpret_cast<const uint32_t*>(smem + (dd->off_out - dd->off_trans));
   d.cls = smem + (dd->off_cls - dd->off_trans);
@@ -741,26 +789,44 @@ __global__ void __launch_bounds__(kBodyThreads, 1) k_body(BodyArgs a) {
     const uint8_t* row = a.tiles + a.grp_base[g] * 16;
     const uint32_t maxu = __shfl_sync(0xffffffffu, units, 0);
     if (lane == 0) touched += (a.grp_base[g + 1] - a.grp_base[g]) * 16;
-    const uint8_t* const row0 = row;
     d.reset(start);
+    // lim: rows this lane steps through; units, or fewer once its verdicts are decided (0: not live, or decided at the start)
+    uint32_t lim = live ? units : 0;
+    if (kAcc != 3 && live) {
+      uint32_t need = q_need[32];
+      if (alive != all_q) {
+        need = 0;
+        for (uint32_t q = alive; q; q &= q - 1) need |= q_need[__ffs(q) - 1];
+      }
+      dec.reset(need, d.n_acc);
+      if (dec.decided(d)) lim = 0;
+    }
     // software pipeline: the next row's 16 bytes are in flight while this row runs through the DFA
     uint4 cur = make_uint4(0, 0, 0, 0);
-    if (0 < units && live) cur = ldg_stream16(row + lane * 16);
-    for (uint32_t k = 0; k < maxu; ++k) {
-      const uint32_t m = __popc(__ballot_sync(0xffffffffu, k < units));
-      const uint8_t* next_row = row + (uint64_t)m * 16;
-      uint4 nxt = make_uint4(0, 0, 0, 0);
-      if (k + 1 < units && live) nxt = ldg_stream16(next_row + lane * 16);
-      if (k < units && live) {
-        int nb = (int)len - (int)(k * 16);
-        if (nb >= 16) { d.word(cur.x); d.word(cur.y); d.word(cur.z); d.word(cur.w); }
-        else { d.word_partial(cur.x, nb); d.word_partial(cur.y, nb - 4); d.word_partial(cur.z, nb - 8); d.word_partial(cur.w, nb - 12); }
+    if (0 < lim) { cur = ldg_stream16(row + lane * 16); ++rows_read; }
+    for (uint32_t k0 = 0; k0 < maxu;) {
+      const uint32_t k1 = kAcc == 3 || maxu - k0 <= kDecideRows ? maxu : k0 + kDecideRows;
+      bool stop = false;
+      for (uint32_t k = k0; k < k1; ++k) {
+        const uint32_t m = __popc(__ballot_sync(0xffffffffu, k < units));
+        const uint8_t* next_row = row + (uint64_t)m * 16;
+        uint4 nxt = make_uint4(0, 0, 0, 0);
+        if (k + 1 < lim) { nxt = ldg_stream16(next_row + lane * 16); ++rows_read; }
+        if (k < lim) {
+          int nb = (int)len - (int)(k * 16);
+          if (nb >= 16) { d.word(cur.x); d.word(cur.y); d.word(cur.z); d.word(cur.w); }
+          else { d.word_partial(cur.x, nb); d.word_partial(cur.y, nb - 4); d.word_partial(cur.z, nb - 8); d.word_partial(cur.w, nb - 12); }
+        }
+        cur = nxt; row = next_row;
+        // sticky automaton: stop reading this group as soon as every live lane has either matched or ended
+        if (kAcc == 3 && __ballot_sync(0xffffffffu, live && k + 1 < units && d.s != sticky_state) == 0) { stop = true; break; }
       }
-      cur = nxt; row = next_row;
-      // sticky automaton: stop reading this group as soon as every live lane has either matched or ended
-      if (kAcc == 3 && __ballot_sync(0xffffffffu, live && k + 1 < units && d.s != sticky_state) == 0) break;
+      if (stop) break;
+      k0 = k1;
+      // a decided lane steps no further; row k1, already in flight, is dropped.  The group ends when no lane has rows left.
+      if (kAcc != 3 && k1 < lim && dec.decided(d)) lim = k1;
+      if (__ballot_sync(0xffffffffu, k1 < lim) == 0) break;
     }
-    if (lane == 0) bytes_read += (unsigned long long)(row - row0);
     if (live) {
       const uint32_t acc = d.finish(endout);
       uint32_t hit = 0;
@@ -779,6 +845,8 @@ __global__ void __launch_bounds__(kBodyThreads, 1) k_body(BodyArgs a) {
     }
     signal_group_done<kPush>(a, g, lane);
   }
+  unsigned long long bytes_read = 16ull * rows_read;
+  for (int o = 16; o; o >>= 1) bytes_read += __shfl_down_sync(0xffffffffu, bytes_read, o);
   if (lane == 0 && touched) { atomicAdd(a.counter + 1, touched); atomicAdd(a.counter + 3, bytes_read); }
 }
 

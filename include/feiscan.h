@@ -223,7 +223,8 @@ typedef struct fei_scan_timing {
   float head_ms, body_ms, compact_ms, h2d_ms, d2h_ms, total_ms;
   uint32_t kernel_launches;
   uint64_t body_bytes_touched;   /* tile bytes of groups that had at least one live record */
-  uint64_t body_bytes_read;      /* tile bytes the body kernel really requested (a single-pattern scan stops reading a
+  uint64_t body_bytes_read;      /* tile bytes the body kernel really requested (a multi-pattern scan stops reading a
+                                    record once its content verdicts are decided, a single-pattern scan stops reading a
                                     group once all of its records have matched; copies already in flight are counted) */
 } fei_scan_timing;
 int fei_scan_last_timing(const fei_corpus* c, fei_scan_timing* out);

@@ -5,7 +5,9 @@ Replays what a warp of k_body does -- 32 records of one length-sorted group walk
 lane -- on the synthetic corpus and the BASELINE configs[2] pattern batch, and counts, per warp-wide lookup, the conflict degree of
 the 32 addresses (max number of distinct 4-byte words that fall into one of the 32 banks = shared-memory wavefronts) for a number
 of table layouts.  Also prints the state-occupancy histogram and how compressible the transition table is.  The measured figure
-of the shipped layout (ncu: 3.26-3.4 wavefronts per lookup) is reproduced by the first line.
+of the shipped layout (ncu: 3.26-3.4 wavefronts per lookup) is reproduced by the first line.  The last section replays a
+per-lane early exit for k_body (a lane stops once its content verdicts are decided) over the groups of one window; DESIGN
+5.1 gives what it measured on the GPU.
 
     python tools/sim_lookup.py [groups]
 """
@@ -139,6 +141,64 @@ def main():
         per = 1.0 if copies >= 32 else 2.0 if copies >= 16 else 2.9 if copies >= 8 else 3.2
         print(f"  {k} sub-automata of {32 // k} patterns: {states} states, class-indexed {'u8' if u8 else 'u16'} tables {kb:.1f} KB together -> at most {copies} bank-confined copies "
               f"(~{per:.1f} wavefronts per lookup), but {k} lookups per byte = ~{k * per:.1f} wavefronts per byte (plus the byte -> class lookup)")
+
+    early_exit_model(d, recs, order, tile_perm)
+
+
+def early_exit_model(d, recs, order, tile_perm):
+    """A per-lane early exit for k_body, replayed on the 128 groups of window 0: a lane stops at the end of the 16-byte row in which the
+    out[] masks of the states it has visited cover every content bit its queries read (all 32 here).  Counts, with and
+    without the exit, the record bytes stepped through the automaton, the warp steps (16 per row in which some lane is
+    still stepping) and the LDS wavefronts of the shipped layout, counting only the lanes that step."""
+    need = (1 << d.n_patterns) - 1
+    lanes = np.arange(32)
+    tot = {"bytes": [0, 0], "steps": [0, 0], "wavefronts": [0, 0], "lookups": [0, 0]}
+    early = n_rec = 0
+    for g in range(len(order) // 32):
+        ids = order[32 * g:32 * g + 32]
+        lens = np.array([len(recs[i]) for i in ids])
+        L = int(lens.max())
+        B = np.zeros((L, 32), dtype=np.int64)
+        for j, i in enumerate(ids):
+            B[:lens[j], j] = np.frombuffer(recs[i], dtype=np.uint8)
+        S = np.zeros((L, 32), dtype=np.int64)                        # state before byte t
+        s = np.full(32, d.start)
+        acc = np.full(32, int(d.out[d.start]), dtype=np.int64)
+        done_at = np.full(32, -1)                                    # first byte after which acc covers need
+        for t in range(L):
+            S[t] = s
+            s = d.trans[s, B[t]]
+            acc |= d.out[s].astype(np.int64)
+            newly = (done_at < 0) & ((acc & need) == need) & (t < lens)
+            done_at[newly] = t
+        rows = (lens + 15) // 16
+        stop_rows = np.where(done_at >= 0, done_at // 16 + 1, rows)  # rows a lane runs with the exit
+        n_rec += 32
+        early += int((stop_rows < rows).sum())
+        word = S * 129 + tile_perm(B) // 2
+        t = np.arange(L)[:, None]
+        for k, lane_rows in enumerate((rows, stop_rows)):
+            active = (t < lens[None, :]) & (t < 16 * lane_rows[None, :])
+            tot["bytes"][k] += int(active.sum())
+            tot["steps"][k] += 16 * int(lane_rows.max())
+            w = np.where(active, word, -1 - lanes[None, :])          # inactive lanes: distinct negative words, no bank
+            srt = np.sort(w, axis=1)
+            first = np.ones_like(srt, dtype=bool)
+            first[:, 1:] = srt[:, 1:] != srt[:, :-1]
+            first &= srt >= 0
+            cnt = np.zeros((L, 32), dtype=np.int64)
+            r_idx, c_idx = np.nonzero(first)
+            np.add.at(cnt, (r_idx, srt[r_idx, c_idx] % 32), 1)
+            deg = cnt.max(axis=1)
+            tot["wavefronts"][k] += int(deg.sum())
+            tot["lookups"][k] += int((deg > 0).sum())
+    ratio = {k: v[1] / v[0] for k, v in tot.items()}
+    print(f"per-lane early exit model (all {d.n_patterns} content bits needed; window 0, {len(order) // 32} groups in tiler order):")
+    print(f"  records decided before their last row: {early / n_rec:.3f}")
+    print(f"  lane-bytes through the automaton: {ratio['bytes']:.3f} of the full scan")
+    print(f"  LDS wavefronts (active lanes only, byte-indexed u16 rows 129 words apart): {ratio['wavefronts']:.3f} of the full scan "
+          f"({tot['wavefronts'][0] / tot['lookups'][0]:.2f} -> {tot['wavefronts'][1] / tot['lookups'][1]:.2f} per warp-wide lookup)")
+    print(f"  warp steps: {ratio['steps']:.3f} of the full scan")
 
 
 if __name__ == "__main__":
