@@ -54,7 +54,8 @@ class CorpusStats(C.Structure):
 class ScanTiming(C.Structure):
     _fields_ = [("head_ms", C.c_float), ("body_ms", C.c_float), ("compact_ms", C.c_float), ("h2d_ms", C.c_float),
                 ("d2h_ms", C.c_float), ("total_ms", C.c_float), ("kernel_launches", C.c_uint32),
-                ("body_bytes_touched", C.c_uint64), ("body_bytes_read", C.c_uint64)]
+                ("body_bytes_touched", C.c_uint64), ("body_bytes_read", C.c_uint64),
+                ("body_kernel", C.c_uint32), ("body_direct", C.c_uint32), ("body_acc_mode", C.c_uint32)]
 
 
 class DirlistView(C.Structure):

@@ -1544,6 +1544,9 @@ int run_scan(fei_corpus* c, const uint8_t* prog, uint64_t prog_len, int compact_
     direct = d.n_cols == 256;
     sticky_kernel = direct && acc_mode == 3 && (uint64_t)d.n_states * d.row_stride * 2 + kStickyAddrSlack <= kStickyAddrLimit;
     gather = sticky_kernel && need_head && n >= 65536;         // few survivors of the header pass: one thread per record (device-side choice)
+    c->timing.body_kernel = gather ? 2u : sticky_kernel ? 1u : 3u;     // gather: finish_timing settles it from the live count
+    c->timing.body_direct = direct ? 1u : 0u;
+    c->timing.body_acc_mode = (uint32_t)acc_mode;
   } else if (n && !need_head) {
     // no condition reads the corpus at all (constant queries): every record gets the constant verdict
     // (program.py folds constants into head conditions, so this only happens for empty condition lists)
@@ -1660,6 +1663,7 @@ int finish_timing(fei_corpus* c, bool compacted) {
   FEI_CUDA(cudaMemcpy(cnt, c->work_counter.as<unsigned long long>(), sizeof(cnt), cudaMemcpyDeviceToHost));
   c->timing.body_bytes_touched = cnt[1];
   c->timing.body_bytes_read = cnt[3];
+  if (c->timing.body_kernel == 2u && cnt[4] > c->n / kGatherDiv) c->timing.body_kernel = 1u;   // k_body_sticky took the dense case
   if (cnt[5]) { set_error("pipelined scan: the side stream gave up waiting for the scan kernel's finished windows"); return FEI_E_CUDA; }
   return FEI_OK;
 }

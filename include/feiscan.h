@@ -218,7 +218,9 @@ int fei_scan_fetch_hits(fei_corpus* c, uint32_t nq, uint64_t* const* hits, const
 int fei_scan_list_checksum(fei_corpus* c, uint32_t nq, uint64_t* a, uint64_t* s);
 
 /* Per-call timing of the last scan on this corpus, measured with CUDA events on the
- * launching stream: ms spent in the head kernel, body kernel, compaction, copies.    */
+ * launching stream: ms spent in the head kernel, body kernel, compaction, copies, and which
+ * content-scan kernel ran.  fei_b200/_abi.py (ScanTiming) is the only consumer of this
+ * struct; fields are only ever appended.                                                    */
 typedef struct fei_scan_timing {
   float head_ms, body_ms, compact_ms, h2d_ms, d2h_ms, total_ms;
   uint32_t kernel_launches;
@@ -226,6 +228,13 @@ typedef struct fei_scan_timing {
   uint64_t body_bytes_read;      /* tile bytes the body kernel really requested (a multi-pattern scan stops reading a
                                     record once its content verdicts are decided, a single-pattern scan stops reading a
                                     group once all of its records have matched; copies already in flight are counted) */
+  uint32_t body_kernel;          /* 0 no content pass, 1 k_body_sticky, 2 k_body_gather, 3 k_body.  The sticky / gather choice
+                                    is made on the device from the records left alive by the header conditions: 2 when at most
+                                    1 in 16 are; also 2 when none is, in which case neither kernel reads a byte
+                                    (body_bytes_read == 0) */
+  uint32_t body_direct;          /* content automaton rows: 1 byte-indexed, 0 class-indexed */
+  uint32_t body_acc_mode;        /* how k_body records accepting states: 1 / 2 <= 32 / <= 64 of them as register bits,
+                                    0 out[] per step, 3 single-pattern (sticky) automaton */
 } fei_scan_timing;
 int fei_scan_last_timing(const fei_corpus* c, fei_scan_timing* out);
 
