@@ -62,14 +62,14 @@ struct fei_corpus {
   fei::DevBuf aux[FEI_MAX_AUX]; uint64_t aux_n[FEI_MAX_AUX] = {0};   // host-computed per-record verdict bytes (fei_corpus_set_aux, FEI_C_RECBITS)
   fei::DevBuf stage_raw, stage_raw_off, stage_ms, stage_hlen, stage_blen;   // raw ingest staging (ingest.cu)
   // scan scratch (grown on demand, reused across scans)
-  fei::DevBuf prog, hits, hit_lists, work_counter, scan_tmp, survivors, live_list, win_done;
+  fei::DevBuf prog, hits, hit_lists, work_counter, scan_tmp, survivors, live_list, win_done, win_state;
   fei::CompactScratch compact;
   uint64_t hit_list_stride = 0;          // entries per query in hit_lists (last fei_scan_hits)
   uint32_t last_nq = 0;
   uint64_t last_counts[32] = {0};
   fei_scan_timing timing = {};
   cudaEvent_t ev[8] = {nullptr};
-  // chunked scans: compaction / all-gather of a finished chunk run on `side` under the next chunk's scan (scan.cu)
+  // chunked scans: compaction (single-pattern scans) / all-gather of a finished chunk run on `side` under the next chunk's scan (scan.cu)
   cudaStream_t side = nullptr;
   cudaEvent_t ev_load[3] = {nullptr, nullptr, nullptr};   // load_raw: before / after the text copy, end of the pack kernels
   bool load_timed = false; uint64_t load_raw_bytes = 0;

@@ -20,8 +20,12 @@
 //          its own record through the multi-pattern DFA whose tables were staged into shared
 //          memory with 1-D TMA bulk copies (cp.async.bulk + mbarrier).  Groups with no live
 //          record are skipped without touching their bytes.  hits[i] = alive[i] & content bits.
+//          The warp that completes a window of 4096 records also appends the window's hits to the
+//          per-query ordered lists (build_window_lists: decoupled look-back over the windows); warps
+//          with no group left help write the last windows' lists (help_tail).
 // k_count / k_scan_blocks / k_emit : order-preserving compaction of hits[] into per-query lists
-//          of global record indices (warp ballots + popc prefix, block offsets from a scan).
+//          of global record indices (warp ballots + popc prefix, block offsets from a scan), for
+//          the single-pattern kernels, header-only programs and gathered multi-GPU masks.
 #include "corpus.h"
 #include "../../include/feiscan_prog.h"
 #include "pyws.cuh"
@@ -592,6 +596,10 @@ struct BodyArgs {
   // of the next ones, from inside the scan kernel.  push_peers is a DEVICE array (a dynamic index into this by-value struct would
   // make ptxas copy it to local memory).
   uint32_t* const* push_peers; uint32_t push_n; unsigned long long push_off, n_records;
+  // ordered hit lists (k_body): the warp that completes a window also writes the window's part of every query's list
+  // (build_window_lists); win_state holds kWinBytes of look-back / emit state per window, zeroed once per scan
+  uint64_t* lists; unsigned long long list_stride, list_base;
+  unsigned long long* totals; uint8_t* win_state; uint32_t nq;
 };
 constexpr uint32_t kGroupsPerWindow = kWindow / 32;
 __device__ __noinline__ void publish_window(const uint32_t* __restrict__ hits, uint32_t* const* __restrict__ peers, uint32_t n_peers,
@@ -615,18 +623,194 @@ __device__ __noinline__ void publish_window(const uint32_t* __restrict__ hits, u
   }
   __threadfence_system();                            // the remote stores are ordered before this kernel's completion is observed
 }
+// ---- ordered hit lists: the per-32-record pieces of the compaction, shared by k_count / k_emit and build_window_lists
+// lane q (< nq) gets the number of the warp's 32 masks that have bit q
+__device__ __forceinline__ uint32_t count_hits32(uint32_t m, uint32_t nq, int lane) {
+  uint32_t cnt = 0;
+#pragma unroll 8
+  for (uint32_t q = 0; q < nq; ++q) {                // unrolled: independent ballots in flight together
+    const uint32_t b = __popc(__ballot_sync(0xffffffffu, (m >> q) & 1u));
+    if (lane == (int)q) cnt = b;
+  }
+  return cnt;
+}
+// query q of the warp's 32 masks in lane order: a lane whose mask has bit q stores `rec` (its global index) at
+// lists[q * stride + pos + hits of the lanes below it]; returns the warp's hits of query q
+__device__ __forceinline__ uint32_t emit_hits32(uint32_t m, uint32_t q, uint64_t pos, uint64_t rec, uint64_t stride, uint64_t* lists, int lane) {
+  const bool hit = (m >> q) & 1u;
+  const uint32_t bal = __ballot_sync(0xffffffffu, hit);
+  if (hit) {
+    const uint64_t rank = pos + __popc(bal & ((1u << lane) - 1u));
+    if (rank < stride) __stcs(reinterpret_cast<unsigned long long*>(lists + q * stride + rank), (unsigned long long)rec);   // nothing reads them back soon
+  }
+  return __popc(bal);
+}
+
+// Per-window state of the list building, one record of kWinBytes per window, zeroed once per scan:
+//   desc[32]  look-back descriptor of (window, query): flag in the top 2 bits over a 62-bit hit count;
+//   ready     set (release) once excl[] and boff[] below are written;   claim: blocks of the window's emit handed out so far;
+//   excl[32]  hits of query q in all earlier windows;   boff[b][32]: hits of query q in the window's records before block b.
+// The emit of a window is cut into kEmitBlocks blocks of kEmitBlockRecs records, claimed one at a time: the completer of the
+// window takes them, and so do warps that find no group left to scan (help_tail), so the last windows' lists are written by
+// many warps instead of one each after the scan ends.
+constexpr unsigned long long kDescAggregate = 1ull << 62, kDescPrefix = 2ull << 62, kDescCount = (1ull << 62) - 1;
+constexpr uint32_t kEmitBlocks = 16, kEmitBlockRecs = kWindow / kEmitBlocks;
+constexpr uint32_t kWinDesc = 0, kWinCtl = 256, kWinExcl = 272, kWinBoff = 528, kWinBytes = kWinBoff + kEmitBlocks * 32 * 4;
+constexpr uint32_t kHelpWindows = 64;              // windows at the end of a launch that warps without a group help with
+__device__ __forceinline__ void st_release_u64(unsigned long long* p, unsigned long long v) {
+  asm volatile("st.release.gpu.global.u64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
+}
+__device__ __forceinline__ unsigned long long ld_acquire_u64(const unsigned long long* p) {
+  unsigned long long v;
+  asm volatile("ld.acquire.gpu.global.u64 %0, [%1];" : "=l"(v) : "l"(p) : "memory");
+  return v;
+}
+__device__ __forceinline__ void st_release_u32(unsigned int* p, unsigned int v) {
+  asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
+}
+__device__ __forceinline__ unsigned int ld_acquire_u32(const unsigned int* p) {
+  unsigned int v;
+  asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
+  return v;
+}
+
+// Claims blocks of window w's emit until none is left and writes each block's hits in record order (the window is ready).
+__device__ __forceinline__ void emit_claimed(const uint32_t* __restrict__ hits, uint8_t* __restrict__ win, uint64_t* __restrict__ lists,
+                                             unsigned long long stride, unsigned long long list_base, unsigned long long n_records,
+                                             uint32_t nq, unsigned long long w, int lane) {
+  uint8_t* wr = win + w * kWinBytes;
+  unsigned int* claim = reinterpret_cast<unsigned int*>(wr + kWinCtl) + 1;
+  const unsigned long long excl = __ldcg(reinterpret_cast<const unsigned long long*>(wr + kWinExcl) + lane);
+  for (;;) {
+    uint32_t b = 0;
+    if (lane == 0) b = atomicAdd(claim, 1u);
+    b = __shfl_sync(0xffffffffu, b, 0);
+    if (b >= kEmitBlocks) break;
+    const unsigned long long r0 = w * kWindow + b * kEmitBlockRecs;
+    if (r0 >= n_records) continue;                   // the last window may be short
+    const uint32_t cnt = (uint32_t)((n_records - r0) < kEmitBlockRecs ? (n_records - r0) : kEmitBlockRecs);
+    const uint32_t* src = hits + r0;
+    // lane q: rank of the next hit of query q (records are 32-bit indices, so a rank fits: one shuffle per query and row of 32)
+    uint32_t pos = (uint32_t)(excl + __ldcg(reinterpret_cast<const unsigned int*>(wr + kWinBoff) + b * 32 + lane));
+    uint32_t nxt = (uint32_t)lane < cnt ? __ldcg(src + lane) : 0u;
+    for (uint32_t i = 0; i < cnt; i += 32) {
+      const uint32_t m = nxt;
+      nxt = i + 32 + lane < cnt ? __ldcg(src + i + 32 + lane) : 0u;
+      const unsigned long long rec = list_base + r0 + i + lane;
+      const uint32_t at = pos;                       // every query reads its rank from the row's start: no chain between queries
+      uint32_t add = 0;
+#pragma unroll 8
+      for (uint32_t q = 0; q < nq; ++q) {
+        const uint32_t n = emit_hits32(m, q, __shfl_sync(0xffffffffu, at, q), rec, stride, lists, lane);
+        if (lane == (int)q) add = n;
+      }
+      pos = at + add;
+    }
+  }
+}
+
+// Window w's part of the ordered per-query lists, started by the warp that completed the window (out of line, like
+// publish_window: the row loop of k_body keeps its register allocation).  Lane q owns query q:
+//   1. count the window's hits block by block (masks of records >= n_records are not read), keep the per-block offsets, and
+//      publish the count as the window's aggregate;
+//   2. decoupled look-back: add up the aggregates of windows w-1, w-2, ... until one carries an inclusive prefix (or window 0
+//      is reached), then publish this window's inclusive prefix, its offsets and `ready`; the last window writes totals[q];
+//   3. emit blocks of the window until every block is claimed (emit_claimed).
+// Progress: a completer publishes its aggregate before it looks back, and it holds no unfinished group (its own group was
+// done when it got here, and it claims the next one only after returning).  Groups are handed out in increasing order and
+// only to resident warps, so every window it waits for is either complete -- its completer publishes the aggregate without
+// waiting for anything -- or has groups that warps still scanning will finish; windows of earlier launches of the same scan
+// are complete.  The time limit only guards against a scan that died: it sets err (reported by finish_timing), and the
+// window publishes its prefix anyway so that later windows do not wait on it too.
+__device__ __noinline__ void build_window_lists(const uint32_t* __restrict__ hits, uint8_t* __restrict__ win, uint64_t* __restrict__ lists,
+                                                unsigned long long stride, unsigned long long list_base, unsigned long long* __restrict__ totals,
+                                                unsigned long long* __restrict__ err, unsigned long long n_records, uint32_t nq,
+                                                unsigned long long w, int lane) {
+  __threadfence();                                   // acquire side of the window counter: the other groups' masks are visible now
+  const unsigned long long r0 = w * kWindow;
+  const uint32_t cnt = (uint32_t)((n_records - r0) < kWindow ? (n_records - r0) : kWindow);
+  const uint32_t* src = hits + r0;
+  const bool own = lane < (int)nq;
+  uint8_t* wr = win + w * kWinBytes;
+  unsigned int* boff = reinterpret_cast<unsigned int*>(wr + kWinBoff);
+  uint32_t agg = 0;
+  uint32_t nxt = (uint32_t)lane < cnt ? __ldcg(src + lane) : 0u;          // L2: other SMs wrote them
+  for (uint32_t i = 0; i < cnt; i += 32) {
+    if ((i & (kEmitBlockRecs - 1)) == 0) boff[(i / kEmitBlockRecs) * 32 + lane] = agg;
+    const uint32_t m = nxt;
+    nxt = i + 32 + lane < cnt ? __ldcg(src + i + 32 + lane) : 0u;
+    agg += count_hits32(m, nq, lane);
+  }
+  unsigned long long* mine = reinterpret_cast<unsigned long long*>(wr + kWinDesc) + lane;
+  unsigned long long excl = 0;
+  if (w == 0) {
+    if (own) st_release_u64(mine, kDescPrefix | agg);
+  } else {
+    if (own) st_release_u64(mine, kDescAggregate | agg);
+    unsigned long long p = w - 1;
+    bool done = !own;
+    const long long t0 = clock64();
+    for (;;) {
+      bool moved = false;
+      if (!done) {
+        const unsigned long long v = ld_acquire_u64(reinterpret_cast<const unsigned long long*>(win + p * kWinBytes + kWinDesc) + lane);
+        if (v >> 62) {
+          excl += v & kDescCount; moved = true;
+          if ((v >> 62) == 2 || p == 0) done = true; else --p;
+        }
+      }
+      if (__all_sync(0xffffffffu, done)) break;
+      if (!__any_sync(0xffffffffu, moved)) {
+        if (clock64() - t0 > 20000000000ll) { if (lane == 0) atomicExch(err, 1ull); break; }     // ~10 s
+        __nanosleep(256);
+      }
+    }
+    if (own) st_release_u64(mine, kDescPrefix | (excl + agg));
+  }
+  if (own && r0 + cnt == n_records) totals[lane] = excl + agg;
+  reinterpret_cast<unsigned long long*>(wr + kWinExcl)[lane] = excl;
+  __threadfence();
+  __syncwarp();
+  if (lane == 0) st_release_u32(reinterpret_cast<unsigned int*>(wr + kWinCtl), 1u);    // offsets published: anyone may emit
+  emit_claimed(hits, win, lists, stride, list_base, n_records, nq, w, lane);
+}
+
+// A warp that finds no group left to scan helps emit the last windows of its launch [w_begin, w_end): the groups of those
+// windows are all handed out, so each becomes ready once its completer has looked back (see build_window_lists); a helper
+// holds no group and waits for nothing else.  Windows whose blocks are all claimed are skipped.
+__device__ __noinline__ void help_tail(const uint32_t* __restrict__ hits, uint8_t* __restrict__ win, uint64_t* __restrict__ lists,
+                                       unsigned long long stride, unsigned long long list_base, unsigned long long* __restrict__ err,
+                                       unsigned long long n_records, uint32_t nq, unsigned long long w_begin, unsigned long long w_end, int lane) {
+  const unsigned long long w0 = w_end - w_begin > kHelpWindows ? w_end - kHelpWindows : w_begin;
+  for (unsigned long long w = w0; w < w_end; ++w) {
+    const unsigned int* ctl = reinterpret_cast<const unsigned int*>(win + w * kWinBytes + kWinCtl);
+    if (__ldcg(ctl + 1) >= kEmitBlocks) continue;                // every block already taken
+    const long long t0 = clock64();
+    while (__any_sync(0xffffffffu, ld_acquire_u32(ctl) == 0u)) {
+      if (clock64() - t0 > 20000000000ll) { if (lane == 0) atomicExch(err, 1ull); return; }    // ~10 s
+      __nanosleep(512);
+    }
+    emit_claimed(hits, win, lists, stride, list_base, n_records, nq, w, lane);
+  }
+}
+
 // kPush: the multi-GPU instantiation; the single-GPU kernels do not carry the exchange code (it cost 0.5 % of the headline
-// when it was compiled into the one kernel: a shuffle and a branch per group, and a different register allocation)
-template <bool kPush>
+// when it was compiled into the one kernel: a shuffle and a branch per group, and a different register allocation).
+// kLists: k_body, which builds the ordered hit lists window by window when a.lists is set.
+template <bool kPush, bool kLists>
 __device__ __forceinline__ void signal_group_done(const BodyArgs& a, unsigned long long g, int lane) {
   if (!a.win_done) return;
   __threadfence();                                   // this lane's hit mask is visible device-wide ...
   __syncwarp();
   unsigned int old = 0;
   if (lane == 0) old = atomicAdd(a.win_done + g / kGroupsPerWindow, 1u);   // ... before the group counts as done
-  if (kPush && a.push_n) {
+  if ((kPush && a.push_n) || (kLists && a.lists)) {
     old = __shfl_sync(0xffffffffu, old, 0);
-    if (old + 1u == kGroupsPerWindow) publish_window(a.hits, a.push_peers, a.push_n, a.push_off, a.n_records, g / kGroupsPerWindow, lane);
+    if (old + 1u == kGroupsPerWindow) {
+      const unsigned long long w = g / kGroupsPerWindow;
+      if (kPush && a.push_n) publish_window(a.hits, a.push_peers, a.push_n, a.push_off, a.n_records, w, lane);
+      if (kLists && a.lists) build_window_lists(a.hits, a.win_state, a.lists, a.list_stride, a.list_base, a.totals, a.counter + 5, a.n_records, a.nq, w, lane);
+    }
   }
 }
 
@@ -783,7 +967,7 @@ __global__ void __launch_bounds__(kBodyThreads, 1) k_body(BodyArgs a) {
     const bool live = alive != 0;
     if (__ballot_sync(0xffffffffu, live) == 0) {              // nobody in this group can still match: skip its bytes
       if (rec != kInvalidRec && !a.has_alive) a.hits[rec] = 0;
-      signal_group_done<kPush>(a, g, lane);
+      signal_group_done<kPush, true>(a, g, lane);
       continue;
     }
     const uint8_t* row = a.tiles + a.grp_base[g] * 16;
@@ -843,8 +1027,11 @@ __global__ void __launch_bounds__(kBodyThreads, 1) k_body(BodyArgs a) {
     } else if (rec != kInvalidRec && !a.has_alive) {
       a.hits[rec] = 0;
     }
-    signal_group_done<kPush>(a, g, lane);
+    signal_group_done<kPush, true>(a, g, lane);
   }
+  if (a.lists && a.win_done)                       // no group left: help write the lists of this launch's last windows
+    help_tail(a.hits, a.win_state, a.lists, a.list_stride, a.list_base, a.counter + 5, a.n_records, a.nq,
+              a.g_begin / kGroupsPerWindow, a.n_groups / kGroupsPerWindow, lane);
   unsigned long long bytes_read = 16ull * rows_read;
   for (int o = 16; o; o >>= 1) bytes_read += __shfl_down_sync(0xffffffffu, bytes_read, o);
   if (lane == 0 && touched) { atomicAdd(a.counter + 1, touched); atomicAdd(a.counter + 3, bytes_read); }
@@ -1129,8 +1316,8 @@ __global__ void __launch_bounds__(kBodyThreads, 1) k_body_sticky(BodyArgs a) {
     ragged_pair(A, B);
     close_group(A);
     close_group(B);
-    signal_group_done<kPush>(a, g, lane);
-    if (g + 1 < a.n_groups) signal_group_done<kPush>(a, g + 1, lane);
+    signal_group_done<kPush, false>(a, g, lane);
+    if (g + 1 < a.n_groups) signal_group_done<kPush, false>(a, g + 1, lane);
   }
   if (lane == 0 && touched) { atomicAdd(a.counter + 1, touched); atomicAdd(a.counter + 3, bytes_read); }
 }
@@ -1258,11 +1445,7 @@ k_count(const uint32_t* __restrict__ hits, uint64_t n, uint32_t nq, uint64_t blk
   uint32_t cnt = 0;                        // lane q accumulates query q
   for (int r = 0; r < kCompactPer; ++r) {
     uint64_t i = base + (uint64_t)(warp * kCompactPer + r) * 32 + lane;
-    uint32_t m = i < n ? hits[i] : 0u;
-    for (uint32_t q = 0; q < nq; ++q) {
-      uint32_t b = __popc(__ballot_sync(0xffffffffu, (m >> q) & 1u));
-      if (lane == (int)q) cnt += b;
-    }
+    cnt += count_hits32(i < n ? hits[i] : 0u, nq, lane);
   }
   sh[lane][warp] = cnt;
   __syncthreads();
@@ -1303,7 +1486,7 @@ __global__ void k_scan_blocks(const uint32_t* __restrict__ counts, uint64_t blk0
 }
 
 // ordered emit: lists[q * stride + rank] = global_base + i
-// (32 registers: one CTA of it fits next to a 1024-thread scan CTA that leaves 8 K of the SM's registers free)
+// (a resident scan CTA of k_body holds the whole register file, so these kernels run between scans, not under one)
 __global__ void __launch_bounds__(kCompactBlock, 8)
 k_emit(const uint32_t* __restrict__ hits, uint64_t n, uint32_t nq, const uint64_t* __restrict__ offsets, uint64_t blk0,
        uint64_t global_base, uint64_t stride, uint64_t* __restrict__ lists) {
@@ -1316,25 +1499,15 @@ k_emit(const uint32_t* __restrict__ hits, uint64_t n, uint32_t nq, const uint64_
   for (int r = 0; r < kCompactPer; ++r) {
     uint64_t i = base + (uint64_t)(warp * kCompactPer + r) * 32 + lane;
     m[r] = i < n ? hits[i] : 0u;
-    for (uint32_t q = 0; q < nq; ++q) {
-      uint32_t b = __popc(__ballot_sync(0xffffffffu, (m[r] >> q) & 1u));
-      if (lane == (int)q) cnt += b;
-    }
+    cnt += count_hits32(m[r], nq, lane);
   }
   wcnt[warp][lane] = cnt;
   __syncthreads();
   for (uint32_t q = 0; q < nq; ++q) {
     uint64_t pos = offsets[blk * nq + q];
     for (int w = 0; w < warp; ++w) pos += wcnt[w][q];
-    for (int r = 0; r < kCompactPer; ++r) {
-      uint32_t bal = __ballot_sync(0xffffffffu, (m[r] >> q) & 1u);
-      if ((m[r] >> q) & 1u) {
-        uint64_t i = base + (uint64_t)(warp * kCompactPer + r) * 32 + lane;
-        uint64_t rank = pos + __popc(bal & ((1u << lane) - 1u));
-        if (rank < stride) lists[q * stride + rank] = global_base + i;
-      }
-      pos += __popc(bal);
-    }
+    for (int r = 0; r < kCompactPer; ++r)
+      pos += emit_hits32(m[r], q, pos, global_base + base + (uint64_t)(warp * kCompactPer + r) * 32 + lane, stride, lists, lane);
   }
 }
 
@@ -1403,8 +1576,9 @@ static int check_prog(const uint8_t* prog, uint64_t len) {
 
 // ---- chunking: the body pass runs as up to kMaxChunks launches over runs of whole windows (a window = kWindow consecutive
 // records = kWindow / 32 groups, so a chunk's hit masks are one contiguous record range).  The moment a chunk's masks are
-// final its compaction (and the hook, e.g. the NCCL all-gather of comm.cu) is queued on the side stream and runs under the
-// next chunk's scan: the 32-pattern scan is shared-memory bound and leaves three quarters of the HBM bandwidth idle.
+// final the hook (e.g. the NCCL all-gather of comm.cu) and, for the single-pattern kernels, its compaction are queued on the
+// side stream.  k_body builds the ordered lists itself, window by window (build_window_lists): side-stream kernels cannot run
+// under it, since one resident 1024-thread k_body CTA holds the SM's whole register file.
 constexpr uint32_t kMaxChunks = 16;
 struct ChunkPlan { uint32_t n = 1; uint64_t g[kMaxChunks + 1] = {0}; uint64_t rec[kMaxChunks + 1] = {0}; };
 
@@ -1555,15 +1729,20 @@ int run_scan(fei_corpus* c, const uint8_t* prog, uint64_t prog_len, int compact_
     ++launches;
   }
   const uint64_t n_windows = (n + kWindow - 1) / kWindow;
-  const bool side_work = (n && compact_mode != kCompactNone) || hook;
+  // k_body (every multi-pattern scan, and single-pattern ones the sticky kernel cannot take) builds the ordered lists inside the
+  // scan; the other scans compact the finished masks with k_count / k_scan_blocks / k_emit on the side stream
+  const bool body_lists = n && need_body && !sticky_kernel && compact_mode == kCompactLists;
+  const bool side_compact = n && compact_mode == kCompactLists && !body_lists;
+  const bool side_work = side_compact || hook;
   BodyArgs a{c->prog.as<uint8_t>(), c->tiles.as<uint8_t>(), c->grp_base.as<uint64_t>(), c->grp_rec.as<uint32_t>(), c->grp_len.as<uint32_t>(),
              c->n_groups, c->hits.as<uint32_t>(), need_head ? 1 : 0, c->work_counter.as<unsigned long long>(), 0ull, 0ull, nullptr, nullptr};
+  a.n_records = n;
   const unsigned grid = (unsigned)cx.sm_count;
   // One launch, logical chunks: with side work to overlap, the scan kernel is launched ONCE over all groups and publishes finished
   // windows (win_done); the side stream gates each chunk's compaction / exchange on them with k_wait_windows.  Cutting the scan into
   // several LAUNCHES instead (FEI_SCAN_CHUNK_LAUNCHES=1) costs a persistent-kernel tail per launch.
   const bool env_launches = getenv("FEI_SCAN_CHUNK_LAUNCHES") && getenv("FEI_SCAN_CHUNK_LAUNCHES")[0] == '1';
-  const bool chunkable = n && need_body && !gather && side_work;
+  const bool chunkable = n && need_body && !gather && (side_work || body_lists);
   const bool watermark = chunkable && !env_launches;
   ChunkPlan plan;
   plan.n = force_chunks ? force_chunks : chunk_count(n_windows, chunkable, watermark);
@@ -1591,7 +1770,7 @@ int run_scan(fei_corpus* c, const uint8_t* prog, uint64_t prog_len, int compact_
     return FEI_OK;
   };
   auto side_chunk = [&](uint32_t k) -> int {                    // compaction + hook of chunk k, queued on the side stream
-    if (compact_mode == kCompactLists && plan.rec[k + 1] > plan.rec[k]) {
+    if (side_compact && plan.rec[k + 1] > plan.rec[k]) {
       const uint64_t b0 = plan.rec[k] / kCompactRecs, b1 = (plan.rec[k + 1] + kCompactRecs - 1) / kCompactRecs;   // chunk bounds are multiples of kWindow (= 2 blocks)
       k_count<<<(unsigned)(b1 - b0), kCompactBlock, 0, c->side>>>(c->hits.as<uint32_t>(), n, nq, b0, c->compact.blk_counts.as<uint32_t>());
       k_scan_blocks<<<nq, 256, 0, c->side>>>(c->compact.blk_counts.as<uint32_t>(), b0, b1 - b0, nq, c->compact.blk_offsets.as<uint64_t>(), c->compact.totals.as<uint64_t>());
@@ -1612,15 +1791,30 @@ int run_scan(fei_corpus* c, const uint8_t* prog, uint64_t prog_len, int compact_
     launches += 2;
   }
   const bool push = watermark && hook && hook->push_peers && hook->push_n;
-  if (watermark && (plan.n > 1 || push)) {
-    if (push) { a.push_peers = hook->push_peers; a.push_n = hook->push_n; a.push_off = hook->push_off; a.n_records = n; hook->pushed = true; }
+  // per-chunk side work left once the scan kernel has built the lists and pushed the masks itself: the compaction of the
+  // single-pattern kernels and the copy-engine / NCCL exchange
+  const bool chunk_work = side_compact || (hook && !push);
+  const bool one_launch = watermark && (plan.n > 1 || push || body_lists);
+  if (one_launch || body_lists) {                              // window counters (and, for body_lists, descriptors) for the whole scan
     FEI_TRY(c->win_done.ensure((n_windows + 1) * sizeof(unsigned int)));
     FEI_CUDA(cudaMemsetAsync(c->win_done.p, 0, (n_windows + 1) * sizeof(unsigned int), s));
     a.win_done = c->win_done.as<unsigned int>();
-    FEI_CUDA(cudaEventRecord(c->ev_chunk[0], s));              // head pass done, counters zeroed: the side stream may start polling
-    FEI_CUDA(cudaStreamWaitEvent(c->side, c->ev_chunk[0], 0));
+  }
+  if (body_lists) {                                            // the window state persists across the launches of one scan
+    FEI_TRY(c->win_state.ensure(n_windows * kWinBytes));
+    FEI_CUDA(cudaMemsetAsync(c->win_state.p, 0, n_windows * kWinBytes, s));
+    a.win_state = c->win_state.as<uint8_t>();
+    a.lists = c->hit_lists.as<uint64_t>(); a.list_stride = c->hit_list_stride; a.list_base = c->global_base;
+    a.totals = c->compact.totals.as<unsigned long long>(); a.nq = nq;
+  }
+  if (one_launch) {
+    if (push) { a.push_peers = hook->push_peers; a.push_n = hook->push_n; a.push_off = hook->push_off; hook->pushed = true; }
+    if (chunk_work) {
+      FEI_CUDA(cudaEventRecord(c->ev_chunk[0], s));            // head pass done, counters zeroed: the side stream may start polling
+      FEI_CUDA(cudaStreamWaitEvent(c->side, c->ev_chunk[0], 0));
+    }
     FEI_TRY(launch_body_range(0, c->n_groups, 0));
-    for (uint32_t k = 0; k < plan.n; ++k) {
+    for (uint32_t k = 0; chunk_work && k < plan.n; ++k) {
       const uint64_t w0 = plan.rec[k] / kWindow, w1 = (plan.rec[k + 1] + kWindow - 1) / kWindow;
       if (w1 > w0) { k_wait_windows<<<1, 32, 0, c->side>>>(c->win_done.as<unsigned int>(), w0, w1, a.counter + 5); ++launches; }
       FEI_TRY(side_chunk(k));
@@ -1628,7 +1822,7 @@ int run_scan(fei_corpus* c, const uint8_t* prog, uint64_t prog_len, int compact_
   } else {
     for (uint32_t k = 0; k < plan.n; ++k) {
       if (n && need_body && plan.g[k + 1] > plan.g[k]) FEI_TRY(launch_body_range(plan.g[k], plan.g[k + 1], k));
-      if (!side_work) continue;
+      if (!chunk_work) continue;
       FEI_CUDA(cudaEventRecord(c->ev_chunk[k], s));
       FEI_CUDA(cudaStreamWaitEvent(c->side, c->ev_chunk[k], 0));
       FEI_TRY(side_chunk(k));
@@ -1636,7 +1830,10 @@ int run_scan(fei_corpus* c, const uint8_t* prog, uint64_t prog_len, int compact_
   }
   FEI_CUDA(cudaEventRecord(c->ev[3], s));
   if (side_work) {
-    if (hook) FEI_TRY(hook->on_done(c->side));
+    if (hook) {
+      FEI_CUDA(cudaStreamWaitEvent(c->side, c->ev[3], 0));   // the totals are final (k_body writes them with the last window)
+      FEI_TRY(hook->on_done(c->side));
+    }
     FEI_CUDA(cudaEventRecord(c->ev_side, c->side));
     FEI_CUDA(cudaStreamWaitEvent(s, c->ev_side, 0));
   }
@@ -1664,7 +1861,7 @@ int finish_timing(fei_corpus* c, bool compacted) {
   c->timing.body_bytes_touched = cnt[1];
   c->timing.body_bytes_read = cnt[3];
   if (c->timing.body_kernel == 2u && cnt[4] > c->n / kGatherDiv) c->timing.body_kernel = 1u;   // k_body_sticky took the dense case
-  if (cnt[5]) { set_error("pipelined scan: the side stream gave up waiting for the scan kernel's finished windows"); return FEI_E_CUDA; }
+  if (cnt[5]) { set_error("pipelined scan: a wait for the scan kernel's finished windows timed out"); return FEI_E_CUDA; }
   return FEI_OK;
 }
 

@@ -205,8 +205,10 @@ int fei_scan_masks(fei_corpus* c, const uint8_t* prog, uint64_t prog_len, uint32
 int fei_scan_hits(fei_corpus* c, const uint8_t* prog, uint64_t prog_len,
                   uint64_t* const* hits, const uint64_t* cap, uint64_t* nhits);
 /* Counts on the host, the ordered lists stay on the device: nhits[q] for every query.
- * Big content scans run as a few chunks of whole 4096-record windows; the compaction of a
- * finished chunk runs on a second stream under the next chunk's scan.                  */
+ * The multi-pattern body kernel builds the lists itself while it scans: the warp that
+ * completes a 4096-record window writes that window's part of every list (warps that have
+ * nothing left to scan help with the last windows).  Single-pattern
+ * content scans and header-only programs compact the finished masks with separate kernels. */
 int fei_scan_count(fei_corpus* c, const uint8_t* prog, uint64_t prog_len, uint64_t* nhits);
 /* Copies the lists the last fei_scan_count left on the device (hits[q] has room for cap[q]
  * entries; FEI_E_CAPACITY if one is shorter than its list): the second half of fei_scan_hits
@@ -219,8 +221,10 @@ int fei_scan_list_checksum(fei_corpus* c, uint32_t nq, uint64_t* a, uint64_t* s)
 
 /* Per-call timing of the last scan on this corpus, measured with CUDA events on the
  * launching stream: ms spent in the head kernel, body kernel, compaction, copies, and which
- * content-scan kernel ran.  fei_b200/_abi.py (ScanTiming) is the only consumer of this
- * struct; fields are only ever appended.                                                    */
+ * content-scan kernel ran.  body_ms includes the ordered lists k_body builds; compact_ms is
+ * whatever is left after the body kernel (for k_body scans little more than the copy of the
+ * per-query totals, else the compaction kernels' tail).  fei_b200/_abi.py (ScanTiming) is
+ * the only consumer of this struct; fields are only ever appended.                          */
 typedef struct fei_scan_timing {
   float head_ms, body_ms, compact_ms, h2d_ms, d2h_ms, total_ms;
   uint32_t kernel_launches;
