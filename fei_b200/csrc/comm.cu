@@ -15,7 +15,6 @@
 
 namespace fei {
 namespace {
-constexpr uint32_t kMaxHookChunks = 16;
 void unbind();
 
 typedef struct { char internal[128]; } ncclUniqueId;
@@ -42,8 +41,7 @@ struct Nccl {
   std::mutex mu;                 // one collective at a time per communicator
   // ---- bound shard set (fei_comm_bind_corpus): record count / first global index of every rank's shard, the rank-major
   // buffer every rank receives the all-gathered hit masks in, and that buffer of every peer mapped into this process
-  // (CUDA IPC over NVLink / NVSwitch peer memory) so that a finished chunk of masks goes out with copy-engine transfers
-  // while the SMs keep scanning
+  // (CUDA IPC over NVLink / NVSwitch peer memory) so that the scan kernel can store its finished windows of masks into it
   fei_corpus* bound = nullptr;
   std::vector<uint64_t> shard_n, shard_base;
   uint64_t n_max = 0, n_total = 0;
@@ -88,38 +86,32 @@ void unbind() {
   g.peer_masks.clear(); g.bound = nullptr; g.p2p = false;
 }
 
-// Chunk hook of the pipelined scan: the masks of the chunk go to every rank's rank-major buffer.
-//   p2p  : one cudaMemcpyAsync per peer into the peer's mapped buffer (copy engines; no SM is taken from the scan);
-//   else : grouped ncclBroadcast, one per rank, straight into the final position (the all-gatherv of chunk k).
-struct GatherHook : ChunkHook {
-  fei_corpus* c; uint32_t chunks;
-  int on_chunk(uint32_t k, uint32_t n_chunks, uint64_t rb, uint64_t re, cudaStream_t side) override {
+// After the scan, unless the scan kernel stored its masks into the peers itself, this shard's masks go to every rank's
+// rank-major buffer:
+//   p2p  : one cudaMemcpyAsync per peer into the peer's mapped buffer (copy engines);
+//   else : grouped ncclBroadcast, one per rank, straight into the final position (the all-gatherv of the masks).
+// Then the per-query totals of all ranks; on the p2p paths this all-reduce is also what tells a rank that every peer's
+// stores / copies into its buffer have landed (a rank enters it only after its own, in stream order).
+struct GatherHook : ScanHook {
+  fei_corpus* c;
+  int after_scan(cudaStream_t s) override {
     const int R = g.nranks, me = g.rank;
-    if (g.p2p && pushed) return FEI_OK;                              // the scan kernel stores each finished window into the peers itself
-    if (g.p2p) {
-      if (re > rb)
+    if (g.p2p) {                                                       // (only a p2p scan pushes)
+      if (!pushed && c->n)
         for (int i = 0; i < R; ++i) {
           const int r = (me + i) % R;                                  // every rank starts with a different peer
-          uint32_t* dst = reinterpret_cast<uint32_t*>(g.peer_masks[r]) + (size_t)me * g.n_max + rb;
-          FEI_CUDA(cudaMemcpyAsync(dst, c->hits.as<uint32_t>() + rb, (re - rb) * 4, cudaMemcpyDefault, side));
+          uint32_t* dst = reinterpret_cast<uint32_t*>(g.peer_masks[r]) + (size_t)me * g.n_max;
+          FEI_CUDA(cudaMemcpyAsync(dst, c->hits.as<uint32_t>(), c->n * 4, cudaMemcpyDefault, s));
         }
-      return FEI_OK;
+    } else {
+      FEI_NCCL(g.GroupStart());
+      for (int r = 0; r < R; ++r)
+        if (g.shard_n[r])
+          FEI_NCCL(g.Broadcast(c->hits.as<uint32_t>(), g.gathered_masks.as<uint32_t>() + (size_t)r * g.n_max, g.shard_n[r], ncclUint32, r, g.comm, s));
+      FEI_NCCL(g.GroupEnd());
     }
-    FEI_NCCL(g.GroupStart());
-    for (int r = 0; r < R; ++r) {
-      uint64_t b[kMaxHookChunks + 1];
-      plan_chunks(g.shard_n[r], n_chunks, b);
-      if (b[k + 1] > b[k])
-        FEI_NCCL(g.Broadcast(c->hits.as<uint32_t>() + b[k], g.gathered_masks.as<uint32_t>() + (size_t)r * g.n_max + b[k], b[k + 1] - b[k], ncclUint32, r, g.comm, side));
-    }
-    FEI_NCCL(g.GroupEnd());
-    return FEI_OK;
-  }
-  // per-query totals of all ranks; on the p2p path this all-reduce is also what tells a rank that every peer's copies
-  // into its buffer have landed (a rank enters it only after its own copies, in stream order)
-  int on_done(cudaStream_t side) override {
-    FEI_NCCL(g.AllReduce(c->compact.totals.p, g.totals_dev.p, 32, ncclUint64, ncclSum, g.comm, side));
-    FEI_CUDA(cudaMemcpyAsync(g.totals_host, g.totals_dev.p, 32 * sizeof(uint64_t), cudaMemcpyDeviceToHost, side));
+    FEI_NCCL(g.AllReduce(c->compact.totals.p, g.totals_dev.p, 32, ncclUint64, ncclSum, g.comm, s));
+    FEI_CUDA(cudaMemcpyAsync(g.totals_host, g.totals_dev.p, 32 * sizeof(uint64_t), cudaMemcpyDeviceToHost, s));
     return FEI_OK;
   }
 };
@@ -193,12 +185,12 @@ extern "C" int fei_comm_bind_corpus(fei_corpus* c) {
 
 extern "C" int fei_comm_is_p2p(void) { return g.p2p ? 1 : 0; }
 /* 1 if the last fei_comm_scan_gather exchanged its hit masks with stores from inside the scan kernel (peer memory), 0 if copy
- * engines / NCCL moved them chunk by chunk. */
+ * engines / NCCL moved them after the scan. */
 extern "C" int fei_comm_last_exchange_in_kernel(void) { return g.last_pushed ? 1 : 0; }
 
-// Collective.  Scan + ordered local lists exactly like fei_scan_count, cut into chunks; the masks of a finished chunk
-// travel to every rank while the next chunk is scanned.  On return every rank holds the hit masks of ALL shards
-// (rank-major = global listing order) on its device and the global per-query totals in nhits_total[nq].
+// Collective.  Scan + ordered local lists exactly like fei_scan_count; by default the scan kernel stores each finished
+// window of masks into every rank's buffer while it scans the next ones.  On return every rank holds the hit masks of ALL
+// shards (rank-major = global listing order) on its device and the global per-query totals in nhits_total[nq].
 extern "C" int fei_comm_scan_gather(fei_corpus* c, const uint8_t* prog, uint64_t prog_len, uint64_t* nhits_total) {
   FEI_TRY(require_ready());
   if (!c) { set_error("null corpus"); return FEI_E_BADARG; }
@@ -206,18 +198,12 @@ extern "C" int fei_comm_scan_gather(fei_corpus* c, const uint8_t* prog, uint64_t
   std::lock_guard<std::mutex> lock(g.mu);
   std::lock_guard<std::mutex> clock(c->mu);
   if (g.bound != c || g.shard_n[g.rank] != c->n || g.shard_base[g.rank] != c->global_base) { set_error("corpus is not the one bound with fei_comm_bind_corpus (or it was reloaded since)"); return FEI_E_STATE; }
-  // the same chunk count on every rank: from the longest shard
-  const uint64_t w_max = (g.n_max + kWindow - 1) / kWindow;
-  uint32_t chunks = (uint32_t)(w_max / 80);                    // logical chunks of ONE scan launch (window counters), ~300 k records each
-  if (const char* e = getenv("FEI_SCAN_CHUNKS")) chunks = (uint32_t)atoi(e);
-  if (chunks > kMaxHookChunks) chunks = kMaxHookChunks;
-  if (chunks < 1) chunks = 1;
-  GatherHook hook; hook.c = c; hook.chunks = chunks;
+  GatherHook hook; hook.c = c;
   const char* kp = getenv("FEI_COMM_KERNEL_PUSH");
   if (g.p2p && !(kp && kp[0] == '0')) {                            // fused exchange: peer stores from inside the scan kernel
     hook.push_peers = reinterpret_cast<uint32_t* const*>(g.peer_ptrs.p); hook.push_n = (uint32_t)g.nranks; hook.push_off = (uint64_t)g.rank * g.n_max;
   }
-  FEI_TRY(run_scan(c, prog, prog_len, kScanCompactLists, &hook, chunks));
+  FEI_TRY(run_scan(c, prog, prog_len, kScanCompactLists, &hook));
   g.last_pushed = hook.pushed;
   FEI_TRY(finish_timing(c, true));
   g.last_kind = 1; g.last_nq = c->last_nq; g.last_nmax = g.n_max; g.last_n = g.shard_n; g.last_base = g.shard_base;

@@ -209,12 +209,9 @@ extern "C" int fei_corpus_destroy(fei_corpus* c) {
   if (!c) return FEI_OK;
   { std::lock_guard<std::mutex> lock(c->mu); }       // let a scan that another thread still runs on this handle finish
   cudaStreamSynchronize(ctx().stream);
-  if (c->side) { cudaStreamSynchronize(c->side); cudaStreamDestroy(c->side); }
   if (c->load_stream) { cudaStreamSynchronize(c->load_stream); cudaStreamDestroy(c->load_stream); }
   for (auto& e : c->ev_load) if (e) cudaEventDestroy(e);
   for (auto& e : c->ev) if (e) cudaEventDestroy(e);
-  for (auto& e : c->ev_chunk) if (e) cudaEventDestroy(e);
-  if (c->ev_side) cudaEventDestroy(c->ev_side);
   delete c;
   return FEI_OK;
 }

@@ -69,14 +69,10 @@ struct fei_corpus {
   uint64_t last_counts[32] = {0};
   fei_scan_timing timing = {};
   cudaEvent_t ev[8] = {nullptr};
-  // chunked scans: compaction (single-pattern scans) / all-gather of a finished chunk run on `side` under the next chunk's scan (scan.cu)
-  cudaStream_t side = nullptr;
   cudaEvent_t ev_load[3] = {nullptr, nullptr, nullptr};   // load_raw: before / after the text copy, end of the pack kernels
   bool load_timed = false; uint64_t load_raw_bytes = 0;
   uint64_t staged_text_bytes = ~0ull;    // size of the text fei_corpus_stage_text is filling stage_raw with (~0: none)
   cudaStream_t load_stream = nullptr;    // loads of this handle (H2D + pack kernels): own stream, so that batches streamed through several handles overlap
-  cudaEvent_t ev_chunk[16] = {nullptr};
-  cudaEvent_t ev_side = nullptr;
 };
 
 namespace fei {
@@ -87,22 +83,20 @@ int build_tiles(fei_corpus* c, const uint8_t* d_body, const uint64_t* d_body_off
 // builds the header directory from hdr / hdr_off already on the device (hdir.cu)
 int build_header_dir(fei_corpus* c, cudaStream_t s);
 int exclusive_scan_u32_u64(const uint32_t* in, uint64_t n, uint64_t* out, DevBuf& tmp, cudaStream_t s);
-// Hook of a chunked scan: on_chunk is called on the host right after the work that makes the hit masks of records
-// [rec_begin, rec_end) final has been queued, with `side` already waiting for it; on_done after the last chunk.
-struct ChunkHook {
-  // multi-GPU: if set, the scan kernel itself stores every finished window's hit masks into these peer buffers (device array of
-  // push_n pointers, one per rank incl. this one; this rank's records start at element push_off of each).  run_scan sets `pushed`
-  // when the launch it queued does that (k_body / k_body_sticky with window counters); otherwise on_chunk must move the masks.
+// Multi-GPU exchange of a scan (comm.cu).
+struct ScanHook {
+  // if set, the scan kernel itself stores every finished window's hit masks into these peer buffers (device array of push_n
+  // pointers, one per rank incl. this one; this rank's records start at element push_off of each).  run_scan sets `pushed`
+  // when the kernel it launched does that (k_body / k_body_sticky); otherwise after_scan must move the masks.
   uint32_t* const* push_peers = nullptr; uint32_t push_n = 0; uint64_t push_off = 0; bool pushed = false;
-  virtual int on_chunk(uint32_t k, uint32_t n_chunks, uint64_t rec_begin, uint64_t rec_end, cudaStream_t side) = 0;
-  virtual int on_done(cudaStream_t side) { return FEI_OK; }
-  virtual ~ChunkHook() {}
+  // called on the host once the scan, its ordered lists and totals included, has been queued on s
+  virtual int after_scan(cudaStream_t s) = 0;
+  virtual ~ScanHook() {}
 };
 enum { kScanCompactNone = 0, kScanCompactLists = 1 };
-// queues a whole scan (nothing waits for the GPU); force_chunks = 0 lets the scan pick its chunking.  Caller holds c->mu.
-int run_scan(fei_corpus* c, const uint8_t* prog, uint64_t prog_len, int compact_mode, ChunkHook* hook, uint32_t force_chunks);
+// queues a whole scan (nothing waits for the GPU).  Caller holds c->mu.
+int run_scan(fei_corpus* c, const uint8_t* prog, uint64_t prog_len, int compact_mode, ScanHook* hook);
 int finish_timing(fei_corpus* c, bool compacted);
-void plan_chunks(uint64_t n, uint32_t chunks, uint64_t* rec_bounds /* chunks + 1 */);
 int compact_segments(const uint32_t* masks, uint64_t seg_stride, const uint64_t* seg_n, const uint64_t* seg_base, uint32_t n_seg, uint32_t nq,
                      CompactScratch& sc, uint64_t stride, uint64_t* lists, uint64_t* totals_out, cudaStream_t s);
 int list_checksum(const uint64_t* list, uint64_t count, DevBuf& tmp, uint64_t* a_out, uint64_t* s_out, cudaStream_t s);

@@ -582,14 +582,11 @@ struct BodyArgs {
   uint32_t* hits;              // in: alive masks (when has_alive), out: final hit masks
   int has_alive;
   unsigned long long* counter; // [1] = tile bytes of the groups entered, [3] = tile bytes requested (k_body: 16 per lane and
-                               // row it loaded), [4] = live records (gather)
+                               // row it loaded), [4] = live records (gather), [5] = set when a list-building wait timed out
   unsigned long long gather_max;   // k_body_sticky stands down (and k_body_gather runs) when 0 < counter[4] <= gather_max
-  // one launch covers the groups [g_begin, n_groups): the scan is cut into chunks of whole windows so that the compaction
-  // (and, multi-GPU, the all-gather) of a finished chunk overlaps the next chunk's scan; *next hands out the chunk's groups
-  unsigned long long g_begin;
-  unsigned long long* next;
-  // window w (groups [w * kWindow / 32, (w + 1) * kWindow / 32)) is finished when win_done[w] reaches kWindow / 32: the side stream
-  // waits on these counters (k_wait_windows) to compact / send a finished run of windows while this kernel is still scanning
+  unsigned long long* next;    // hands out the groups [0, n_groups) of the one launch
+  // window w (groups [w * kWindow / 32, (w + 1) * kWindow / 32)) is finished when win_done[w] reaches kWindow / 32; null unless
+  // the warp that finishes a window has work to do for it (ordered lists, peer push)
   unsigned int* win_done;
   // multi-GPU, fused exchange: the warp that completes a window stores the window's 4096 hit masks into every rank's rank-major
   // mask buffer (peer memory over NVLink / NVSwitch, mapped with CUDA IPC) -- the transfer of a finished window runs under the scan
@@ -656,7 +653,7 @@ __device__ __forceinline__ uint32_t emit_hits32(uint32_t m, uint32_t q, uint64_t
 constexpr unsigned long long kDescAggregate = 1ull << 62, kDescPrefix = 2ull << 62, kDescCount = (1ull << 62) - 1;
 constexpr uint32_t kEmitBlocks = 16, kEmitBlockRecs = kWindow / kEmitBlocks;
 constexpr uint32_t kWinDesc = 0, kWinCtl = 256, kWinExcl = 272, kWinBoff = 528, kWinBytes = kWinBoff + kEmitBlocks * 32 * 4;
-constexpr uint32_t kHelpWindows = 64;              // windows at the end of a launch that warps without a group help with
+constexpr uint32_t kHelpWindows = 64;              // windows at the end of the scan that warps without a group help with
 __device__ __forceinline__ void st_release_u64(unsigned long long* p, unsigned long long v) {
   asm volatile("st.release.gpu.global.u64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
 }
@@ -719,8 +716,8 @@ __device__ __forceinline__ void emit_claimed(const uint32_t* __restrict__ hits, 
 // Progress: a completer publishes its aggregate before it looks back, and it holds no unfinished group (its own group was
 // done when it got here, and it claims the next one only after returning).  Groups are handed out in increasing order and
 // only to resident warps, so every window it waits for is either complete -- its completer publishes the aggregate without
-// waiting for anything -- or has groups that warps still scanning will finish; windows of earlier launches of the same scan
-// are complete.  The time limit only guards against a scan that died: it sets err (reported by finish_timing), and the
+// waiting for anything -- or has groups that warps still scanning will finish.
+// The time limit only guards against a scan that died: it sets err (reported by finish_timing), and the
 // window publishes its prefix anyway so that later windows do not wait on it too.
 __device__ __noinline__ void build_window_lists(const uint32_t* __restrict__ hits, uint8_t* __restrict__ win, uint64_t* __restrict__ lists,
                                                 unsigned long long stride, unsigned long long list_base, unsigned long long* __restrict__ totals,
@@ -775,14 +772,14 @@ __device__ __noinline__ void build_window_lists(const uint32_t* __restrict__ hit
   emit_claimed(hits, win, lists, stride, list_base, n_records, nq, w, lane);
 }
 
-// A warp that finds no group left to scan helps emit the last windows of its launch [w_begin, w_end): the groups of those
+// A warp that finds no group left to scan helps emit the last windows of the scan [0, n_windows): the groups of those
 // windows are all handed out, so each becomes ready once its completer has looked back (see build_window_lists); a helper
 // holds no group and waits for nothing else.  Windows whose blocks are all claimed are skipped.
 __device__ __noinline__ void help_tail(const uint32_t* __restrict__ hits, uint8_t* __restrict__ win, uint64_t* __restrict__ lists,
                                        unsigned long long stride, unsigned long long list_base, unsigned long long* __restrict__ err,
-                                       unsigned long long n_records, uint32_t nq, unsigned long long w_begin, unsigned long long w_end, int lane) {
-  const unsigned long long w0 = w_end - w_begin > kHelpWindows ? w_end - kHelpWindows : w_begin;
-  for (unsigned long long w = w0; w < w_end; ++w) {
+                                       unsigned long long n_records, uint32_t nq, unsigned long long n_windows, int lane) {
+  const unsigned long long w0 = n_windows > kHelpWindows ? n_windows - kHelpWindows : 0;
+  for (unsigned long long w = w0; w < n_windows; ++w) {
     const unsigned int* ctl = reinterpret_cast<const unsigned int*>(win + w * kWinBytes + kWinCtl);
     if (__ldcg(ctl + 1) >= kEmitBlocks) continue;                // every block already taken
     const long long t0 = clock64();
@@ -956,7 +953,7 @@ __global__ void __launch_bounds__(kBodyThreads, 1) k_body(BodyArgs a) {
 
   for (;;) {
     unsigned long long g = 0;
-    if (lane == 0) g = a.g_begin + atomicAdd(a.next, 1ull);
+    if (lane == 0) g = atomicAdd(a.next, 1ull);
     g = __shfl_sync(0xffffffffu, g, 0);
     if (g >= a.n_groups) break;
     const uint32_t rec = a.grp_rec[g * 32 + lane];
@@ -1029,9 +1026,9 @@ __global__ void __launch_bounds__(kBodyThreads, 1) k_body(BodyArgs a) {
     }
     signal_group_done<kPush, true>(a, g, lane);
   }
-  if (a.lists && a.win_done)                       // no group left: help write the lists of this launch's last windows
+  if (a.lists && a.win_done)                       // no group left: help write the lists of the scan's last windows
     help_tail(a.hits, a.win_state, a.lists, a.list_stride, a.list_base, a.counter + 5, a.n_records, a.nq,
-              a.g_begin / kGroupsPerWindow, a.n_groups / kGroupsPerWindow, lane);
+              a.n_groups / kGroupsPerWindow, lane);
   unsigned long long bytes_read = 16ull * rows_read;
   for (int o = 16; o; o >>= 1) bytes_read += __shfl_down_sync(0xffffffffu, bytes_read, o);
   if (lane == 0 && touched) { atomicAdd(a.counter + 1, touched); atomicAdd(a.counter + 3, bytes_read); }
@@ -1304,7 +1301,7 @@ __global__ void __launch_bounds__(kBodyThreads, 1) k_body_sticky(BodyArgs a) {
 
   for (;;) {
     unsigned long long g = 0;
-    if (lane == 0) g = a.g_begin + atomicAdd(a.next, 2ull);
+    if (lane == 0) g = atomicAdd(a.next, 2ull);
     g = __shfl_sync(0xffffffffu, g, 0);
     if (g >= a.n_groups) break;
     Grp A, B;
@@ -1434,12 +1431,11 @@ constexpr int kCompactBlock = 256;          // threads
 constexpr int kCompactPer = 8;              // records per thread -> 2048 records per block
 constexpr uint64_t kCompactRecs = (uint64_t)kCompactBlock * kCompactPer;
 
-// counts[block * nq + q] = records of this block that hit query q  (block = blk0 + blockIdx.x: a chunk of the scan
-// compacts its own blocks while the next chunk is still being scanned)
+// counts[block * nq + q] = records of this block that hit query q
 __global__ void __launch_bounds__(kCompactBlock)
-k_count(const uint32_t* __restrict__ hits, uint64_t n, uint32_t nq, uint64_t blk0, uint32_t* __restrict__ counts) {
+k_count(const uint32_t* __restrict__ hits, uint64_t n, uint32_t nq, uint32_t* __restrict__ counts) {
   __shared__ uint32_t sh[32][8];
-  const uint64_t blk = blk0 + blockIdx.x;
+  const uint64_t blk = blockIdx.x;
   uint64_t base = blk * kCompactRecs;
   int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   uint32_t cnt = 0;                        // lane q accumulates query q
@@ -1456,9 +1452,9 @@ k_count(const uint32_t* __restrict__ hits, uint64_t n, uint32_t nq, uint64_t blk
   }
 }
 
-// per query: exclusive scan over the blocks [blk0, blk0 + nblocks) (one thread block per query), continuing from
-// carry[q] (the hits of the blocks before blk0) and leaving the new running total there
-__global__ void k_scan_blocks(const uint32_t* __restrict__ counts, uint64_t blk0, uint64_t nblocks, uint32_t nq,
+// per query: exclusive scan over the blocks [0, nblocks) (one thread block per query), continuing from carry[q] (the hits
+// of the segments compacted before this one) and leaving the new running total there
+__global__ void k_scan_blocks(const uint32_t* __restrict__ counts, uint64_t nblocks, uint32_t nq,
                               uint64_t* __restrict__ offsets, uint64_t* __restrict__ carry_io) {
   __shared__ uint64_t sh[1024];
   __shared__ uint64_t carry;
@@ -1467,7 +1463,7 @@ __global__ void k_scan_blocks(const uint32_t* __restrict__ counts, uint64_t blk0
   __syncthreads();
   for (uint64_t base = 0; base < nblocks; base += blockDim.x) {
     uint64_t b = base + threadIdx.x;
-    uint64_t v = b < nblocks ? counts[(blk0 + b) * nq + q] : 0;
+    uint64_t v = b < nblocks ? counts[b * nq + q] : 0;
     sh[threadIdx.x] = v;
     __syncthreads();
     for (int o = 1; o < blockDim.x; o <<= 1) {
@@ -1477,7 +1473,7 @@ __global__ void k_scan_blocks(const uint32_t* __restrict__ counts, uint64_t blk0
       __syncthreads();
     }
     uint64_t incl = sh[threadIdx.x];
-    if (b < nblocks) offsets[(blk0 + b) * nq + q] = carry + incl - v;
+    if (b < nblocks) offsets[b * nq + q] = carry + incl - v;
     __syncthreads();
     if (threadIdx.x == blockDim.x - 1) carry += incl;
     __syncthreads();
@@ -1488,10 +1484,10 @@ __global__ void k_scan_blocks(const uint32_t* __restrict__ counts, uint64_t blk0
 // ordered emit: lists[q * stride + rank] = global_base + i
 // (a resident scan CTA of k_body holds the whole register file, so these kernels run between scans, not under one)
 __global__ void __launch_bounds__(kCompactBlock, 8)
-k_emit(const uint32_t* __restrict__ hits, uint64_t n, uint32_t nq, const uint64_t* __restrict__ offsets, uint64_t blk0,
+k_emit(const uint32_t* __restrict__ hits, uint64_t n, uint32_t nq, const uint64_t* __restrict__ offsets,
        uint64_t global_base, uint64_t stride, uint64_t* __restrict__ lists) {
   __shared__ uint32_t wcnt[8][32];          // [warp][query] hits of this warp's records
-  const uint64_t blk = blk0 + blockIdx.x;
+  const uint64_t blk = blockIdx.x;
   uint64_t base = blk * kCompactRecs;
   int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   uint32_t m[kCompactPer];
@@ -1511,19 +1507,14 @@ k_emit(const uint32_t* __restrict__ hits, uint64_t n, uint32_t nq, const uint64_
   }
 }
 
-// Side-stream gate of a pipelined scan: one warp spins until every window of [w0, w1) is finished (see BodyArgs::win_done).
-// A warp that sleeps between polls costs the scan nothing; the time limit only guards against a scan kernel that died.
-__global__ void k_wait_windows(const volatile unsigned int* __restrict__ win_done, uint64_t w0, uint64_t w1, unsigned long long* __restrict__ err) {
-  const int lane = threadIdx.x & 31;
-  const long long t0 = clock64();
-  for (;;) {
-    bool ok = true;
-    for (uint64_t w = w0 + lane; w < w1; w += 32) ok = ok && win_done[w] >= kGroupsPerWindow;
-    if (__all_sync(0xffffffffu, ok)) break;
-    if (clock64() - t0 > 20000000000ll) { if (lane == 0) atomicExch(err, 1ull); break; }     // ~10 s
-    __nanosleep(1000);
-  }
-  __threadfence();
+// Ordered lists of the n masks at `masks` (record 0 is global index global_base) into lists[q * stride + rank], the ranks
+// continuing from sc.totals, which is left holding the running per-query totals.  n > 0.
+static void compact_lists(const uint32_t* masks, uint64_t n, uint32_t nq, uint64_t global_base, CompactScratch& sc, uint64_t stride,
+                          uint64_t* lists, cudaStream_t s) {
+  const uint64_t nb = (n + kCompactRecs - 1) / kCompactRecs;
+  k_count<<<(unsigned)nb, kCompactBlock, 0, s>>>(masks, n, nq, sc.blk_counts.as<uint32_t>());
+  k_scan_blocks<<<nq, 256, 0, s>>>(sc.blk_counts.as<uint32_t>(), nb, nq, sc.blk_offsets.as<uint64_t>(), sc.totals.as<uint64_t>());
+  k_emit<<<(unsigned)nb, kCompactBlock, 0, s>>>(masks, n, nq, sc.blk_offsets.as<uint64_t>(), global_base, stride, lists);
 }
 
 __global__ void k_fill32(uint32_t* __restrict__ p, uint64_t n, uint32_t v) {
@@ -1574,46 +1565,11 @@ static int check_prog(const uint8_t* prog, uint64_t len) {
 }
 
 
-// ---- chunking: the body pass runs as up to kMaxChunks launches over runs of whole windows (a window = kWindow consecutive
-// records = kWindow / 32 groups, so a chunk's hit masks are one contiguous record range).  The moment a chunk's masks are
-// final the hook (e.g. the NCCL all-gather of comm.cu) and, for the single-pattern kernels, its compaction are queued on the
-// side stream.  k_body builds the ordered lists itself, window by window (build_window_lists): side-stream kernels cannot run
-// under it, since one resident 1024-thread k_body CTA holds the SM's whole register file.
-constexpr uint32_t kMaxChunks = 16;
-struct ChunkPlan { uint32_t n = 1; uint64_t g[kMaxChunks + 1] = {0}; uint64_t rec[kMaxChunks + 1] = {0}; };
-
-static uint32_t chunk_count(uint64_t n_windows, bool allow, bool watermark) {
-  uint32_t want = 0;
-  if (const char* e = getenv("FEI_SCAN_CHUNKS")) want = (uint32_t)atoi(e);
-  if (!allow) return 1;
-  // logical chunks of a single launch are nearly free (a one-warp gate kernel each): ~300 k records and up, at most 16; separate
-  // launches cost a kernel tail each, so without the window counters the scan stays in one piece unless asked otherwise
-  if (!want) want = watermark ? (uint32_t)(n_windows / 80) : 1;
-  if (want > kMaxChunks) want = kMaxChunks;
-  if (want > n_windows) want = (uint32_t)n_windows;
-  return want ? want : 1;
-}
-void plan_chunks(uint64_t n, uint32_t chunks, uint64_t* rec_bounds) {       // shared with comm.cu: every rank derives every rank's bounds
-  const uint64_t n_windows = (n + kWindow - 1) / kWindow;
-  for (uint32_t k = 0; k <= chunks; ++k) { uint64_t r = n_windows * k / chunks * kWindow; rec_bounds[k] = r < n ? r : n; }
-  rec_bounds[chunks] = n;
-}
-
-static int ensure_side(fei_corpus* c) {
-  if (!c->side) {                                              // highest priority: a finished chunk's compaction / all-gather gets the first SM that frees up
-    int lo = 0, hi = 0;
-    FEI_CUDA(cudaDeviceGetStreamPriorityRange(&lo, &hi));
-    FEI_CUDA(cudaStreamCreateWithPriority(&c->side, cudaStreamNonBlocking, hi));
-  }
-  for (auto& e : c->ev_chunk) if (!e) FEI_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-  if (!c->ev_side) FEI_CUDA(cudaEventCreateWithFlags(&c->ev_side, cudaEventDisableTiming));
-  return FEI_OK;
-}
-
 enum { kCompactNone = kScanCompactNone, kCompactLists = kScanCompactLists };
+constexpr int kWorkCounters = 6;           // work_counter: [0] = BodyArgs::next, [2] = header survivors, the rest see BodyArgs::counter
 
-// Everything is queued on the context stream (and the corpus' side stream); nothing here waits for the GPU.
-int run_scan(fei_corpus* c, const uint8_t* prog, uint64_t prog_len, int compact_mode, ChunkHook* hook, uint32_t force_chunks) {
+// Everything is queued on the context stream; nothing here waits for the GPU.
+int run_scan(fei_corpus* c, const uint8_t* prog, uint64_t prog_len, int compact_mode, ScanHook* hook) {
   FEI_TRY(require_ready());
   if (!c || !c->loaded) { set_error("corpus not loaded"); return FEI_E_STATE; }
   FEI_TRY(check_prog(prog, prog_len));
@@ -1626,11 +1582,10 @@ int run_scan(fei_corpus* c, const uint8_t* prog, uint64_t prog_len, int compact_
   for (uint32_t q = 0; q < 32; ++q) c->last_counts[q] = 0;
   FEI_TRY(c->prog.ensure(prog_len + 16));
   FEI_TRY(c->hits.ensure((n ? n : 1) * sizeof(uint32_t)));
-  FEI_TRY(c->work_counter.ensure((8 + kMaxChunks) * sizeof(unsigned long long)));
-  FEI_TRY(ensure_side(c));
+  FEI_TRY(c->work_counter.ensure(kWorkCounters * sizeof(unsigned long long)));
   FEI_CUDA(cudaEventRecord(c->ev[0], s));
   FEI_CUDA(cudaMemcpyAsync(c->prog.p, prog, prog_len, cudaMemcpyHostToDevice, s));
-  FEI_CUDA(cudaMemsetAsync(c->work_counter.p, 0, (8 + kMaxChunks) * sizeof(unsigned long long), s));
+  FEI_CUDA(cudaMemsetAsync(c->work_counter.p, 0, kWorkCounters * sizeof(unsigned long long), s));
   bool need_head = h.head_mask != 0;
   bool need_body = h.off_body_dfa != 0 && h.body_mask != 0;
   if ((h.off_name_dfa[0] || h.off_name_dfa[1] || h.off_name_dfa[2]) && !c->name.p) {
@@ -1706,7 +1661,7 @@ int run_scan(fei_corpus* c, const uint8_t* prog, uint64_t prog_len, int compact_
   }
   FEI_CUDA(cudaEventRecord(c->ev[2], s));
 
-  // ---- body pass, chunk by chunk
+  // ---- body pass: one launch over all groups
   fei_prog_dfa d; memset(&d, 0, sizeof(d));
   size_t smem = 0;
   int acc_mode = 0; bool direct = false, sticky_kernel = false, gather = false;
@@ -1730,29 +1685,37 @@ int run_scan(fei_corpus* c, const uint8_t* prog, uint64_t prog_len, int compact_
   }
   const uint64_t n_windows = (n + kWindow - 1) / kWindow;
   // k_body (every multi-pattern scan, and single-pattern ones the sticky kernel cannot take) builds the ordered lists inside the
-  // scan; the other scans compact the finished masks with k_count / k_scan_blocks / k_emit on the side stream
+  // scan; the other scans compact the finished masks with k_count / k_scan_blocks / k_emit after it
   const bool body_lists = n && need_body && !sticky_kernel && compact_mode == kCompactLists;
-  const bool side_compact = n && compact_mode == kCompactLists && !body_lists;
-  const bool side_work = side_compact || hook;
+  // multi-GPU: the scan kernel stores every finished window's masks into the peers (k_body_gather does not: the hook copies them)
+  const bool push = n && need_body && !gather && hook && hook->push_peers && hook->push_n;
   BodyArgs a{c->prog.as<uint8_t>(), c->tiles.as<uint8_t>(), c->grp_base.as<uint64_t>(), c->grp_rec.as<uint32_t>(), c->grp_len.as<uint32_t>(),
-             c->n_groups, c->hits.as<uint32_t>(), need_head ? 1 : 0, c->work_counter.as<unsigned long long>(), 0ull, 0ull, nullptr, nullptr};
+             c->n_groups, c->hits.as<uint32_t>(), need_head ? 1 : 0, c->work_counter.as<unsigned long long>(), 0ull,
+             c->work_counter.as<unsigned long long>(), nullptr};
   a.n_records = n;
   const unsigned grid = (unsigned)cx.sm_count;
-  // One launch, logical chunks: with side work to overlap, the scan kernel is launched ONCE over all groups and publishes finished
-  // windows (win_done); the side stream gates each chunk's compaction / exchange on them with k_wait_windows.  Cutting the scan into
-  // several LAUNCHES instead (FEI_SCAN_CHUNK_LAUNCHES=1) costs a persistent-kernel tail per launch.
-  const bool env_launches = getenv("FEI_SCAN_CHUNK_LAUNCHES") && getenv("FEI_SCAN_CHUNK_LAUNCHES")[0] == '1';
-  const bool chunkable = n && need_body && !gather && (side_work || body_lists);
-  const bool watermark = chunkable && !env_launches;
-  ChunkPlan plan;
-  plan.n = force_chunks ? force_chunks : chunk_count(n_windows, chunkable, watermark);
-  if (plan.n > kMaxChunks) plan.n = kMaxChunks;
-  if (plan.n < 1) plan.n = 1;
-  plan_chunks(n, plan.n, plan.rec);
-  for (uint32_t k = 0; k <= plan.n; ++k) plan.g[k] = (plan.rec[k] + kWindow - 1) / kWindow * (kWindow / 32);
-  plan.g[plan.n] = c->n_groups;
-  auto launch_body_range = [&](uint64_t g0, uint64_t g1, uint32_t slot) -> int {
-    a.g_begin = g0; a.n_groups = g1; a.next = a.counter + 8 + slot;
+  if (n && need_body && gather) {
+    a.gather_max = n / kGatherDiv;
+    FEI_TRY(c->live_list.ensure((a.gather_max + 1) * sizeof(uint32_t)));
+    k_live_list<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(c->hits.as<uint32_t>(), n, c->live_list.as<uint32_t>(), a.counter + 4, a.gather_max);
+    FEI_CUDA(cudaFuncSetAttribute(k_body_gather, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    k_body_gather<<<grid, kBodyThreads, smem, s>>>(a, c->live_list.as<uint32_t>(), c->rec_pos.as<uint32_t>());
+    launches += 2;
+  }
+  if (body_lists || push) {                                    // window counters (and, for body_lists, descriptors) for the scan
+    FEI_TRY(c->win_done.ensure((n_windows + 1) * sizeof(unsigned int)));
+    FEI_CUDA(cudaMemsetAsync(c->win_done.p, 0, (n_windows + 1) * sizeof(unsigned int), s));
+    a.win_done = c->win_done.as<unsigned int>();
+  }
+  if (body_lists) {
+    FEI_TRY(c->win_state.ensure(n_windows * kWinBytes));
+    FEI_CUDA(cudaMemsetAsync(c->win_state.p, 0, n_windows * kWinBytes, s));
+    a.win_state = c->win_state.as<uint8_t>();
+    a.lists = c->hit_lists.as<uint64_t>(); a.list_stride = c->hit_list_stride; a.list_base = c->global_base;
+    a.totals = c->compact.totals.as<unsigned long long>(); a.nq = nq;
+  }
+  if (push) { a.push_peers = hook->push_peers; a.push_n = hook->push_n; a.push_off = hook->push_off; hook->pushed = true; }
+  if (n && need_body) {
     int rc = FEI_OK;
     if (sticky_kernel) {
       const size_t smem_sticky = ((smem + 127) & ~(size_t)127) + kStickyRingBytes;
@@ -1767,76 +1730,13 @@ int run_scan(fei_corpus* c, const uint8_t* prog, uint64_t prog_len, int compact_
     else rc = acc_mode == 3 ? launch_body<false, 3>(a, grid, smem, s) : acc_mode == 1 ? launch_body<false, 1>(a, grid, smem, s) : acc_mode == 2 ? launch_body<false, 2>(a, grid, smem, s) : launch_body<false, 0>(a, grid, smem, s);
     FEI_TRY(rc);
     ++launches;
-    return FEI_OK;
-  };
-  auto side_chunk = [&](uint32_t k) -> int {                    // compaction + hook of chunk k, queued on the side stream
-    if (side_compact && plan.rec[k + 1] > plan.rec[k]) {
-      const uint64_t b0 = plan.rec[k] / kCompactRecs, b1 = (plan.rec[k + 1] + kCompactRecs - 1) / kCompactRecs;   // chunk bounds are multiples of kWindow (= 2 blocks)
-      k_count<<<(unsigned)(b1 - b0), kCompactBlock, 0, c->side>>>(c->hits.as<uint32_t>(), n, nq, b0, c->compact.blk_counts.as<uint32_t>());
-      k_scan_blocks<<<nq, 256, 0, c->side>>>(c->compact.blk_counts.as<uint32_t>(), b0, b1 - b0, nq, c->compact.blk_offsets.as<uint64_t>(), c->compact.totals.as<uint64_t>());
-      k_emit<<<(unsigned)(b1 - b0), kCompactBlock, 0, c->side>>>(c->hits.as<uint32_t>(), n, nq, c->compact.blk_offsets.as<uint64_t>(), b0, c->global_base,
-                                                               c->hit_list_stride, c->hit_lists.as<uint64_t>());
-      launches += 3;
-    }
-    if (hook) FEI_TRY(hook->on_chunk(k, plan.n, plan.rec[k], plan.rec[k + 1], c->side));
-    return FEI_OK;
-  };
-  if (n && need_body && gather) {
-    a.gather_max = n / kGatherDiv;
-    FEI_TRY(c->live_list.ensure((a.gather_max + 1) * sizeof(uint32_t)));
-    k_live_list<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(c->hits.as<uint32_t>(), n, c->live_list.as<uint32_t>(), a.counter + 4, a.gather_max);
-    FEI_CUDA(cudaFuncSetAttribute(k_body_gather, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    a.next = a.counter + 8;
-    k_body_gather<<<grid, kBodyThreads, smem, s>>>(a, c->live_list.as<uint32_t>(), c->rec_pos.as<uint32_t>());
-    launches += 2;
-  }
-  const bool push = watermark && hook && hook->push_peers && hook->push_n;
-  // per-chunk side work left once the scan kernel has built the lists and pushed the masks itself: the compaction of the
-  // single-pattern kernels and the copy-engine / NCCL exchange
-  const bool chunk_work = side_compact || (hook && !push);
-  const bool one_launch = watermark && (plan.n > 1 || push || body_lists);
-  if (one_launch || body_lists) {                              // window counters (and, for body_lists, descriptors) for the whole scan
-    FEI_TRY(c->win_done.ensure((n_windows + 1) * sizeof(unsigned int)));
-    FEI_CUDA(cudaMemsetAsync(c->win_done.p, 0, (n_windows + 1) * sizeof(unsigned int), s));
-    a.win_done = c->win_done.as<unsigned int>();
-  }
-  if (body_lists) {                                            // the window state persists across the launches of one scan
-    FEI_TRY(c->win_state.ensure(n_windows * kWinBytes));
-    FEI_CUDA(cudaMemsetAsync(c->win_state.p, 0, n_windows * kWinBytes, s));
-    a.win_state = c->win_state.as<uint8_t>();
-    a.lists = c->hit_lists.as<uint64_t>(); a.list_stride = c->hit_list_stride; a.list_base = c->global_base;
-    a.totals = c->compact.totals.as<unsigned long long>(); a.nq = nq;
-  }
-  if (one_launch) {
-    if (push) { a.push_peers = hook->push_peers; a.push_n = hook->push_n; a.push_off = hook->push_off; hook->pushed = true; }
-    if (chunk_work) {
-      FEI_CUDA(cudaEventRecord(c->ev_chunk[0], s));            // head pass done, counters zeroed: the side stream may start polling
-      FEI_CUDA(cudaStreamWaitEvent(c->side, c->ev_chunk[0], 0));
-    }
-    FEI_TRY(launch_body_range(0, c->n_groups, 0));
-    for (uint32_t k = 0; chunk_work && k < plan.n; ++k) {
-      const uint64_t w0 = plan.rec[k] / kWindow, w1 = (plan.rec[k + 1] + kWindow - 1) / kWindow;
-      if (w1 > w0) { k_wait_windows<<<1, 32, 0, c->side>>>(c->win_done.as<unsigned int>(), w0, w1, a.counter + 5); ++launches; }
-      FEI_TRY(side_chunk(k));
-    }
-  } else {
-    for (uint32_t k = 0; k < plan.n; ++k) {
-      if (n && need_body && plan.g[k + 1] > plan.g[k]) FEI_TRY(launch_body_range(plan.g[k], plan.g[k + 1], k));
-      if (!chunk_work) continue;
-      FEI_CUDA(cudaEventRecord(c->ev_chunk[k], s));
-      FEI_CUDA(cudaStreamWaitEvent(c->side, c->ev_chunk[k], 0));
-      FEI_TRY(side_chunk(k));
-    }
   }
   FEI_CUDA(cudaEventRecord(c->ev[3], s));
-  if (side_work) {
-    if (hook) {
-      FEI_CUDA(cudaStreamWaitEvent(c->side, c->ev[3], 0));   // the totals are final (k_body writes them with the last window)
-      FEI_TRY(hook->on_done(c->side));
-    }
-    FEI_CUDA(cudaEventRecord(c->ev_side, c->side));
-    FEI_CUDA(cudaStreamWaitEvent(s, c->ev_side, 0));
+  if (n && compact_mode == kCompactLists && !body_lists) {
+    compact_lists(c->hits.as<uint32_t>(), n, nq, c->global_base, c->compact, c->hit_list_stride, c->hit_lists.as<uint64_t>(), s);
+    launches += 3;
   }
+  if (hook) FEI_TRY(hook->after_scan(s));
   if (compact_mode == kCompactLists)
     FEI_CUDA(cudaMemcpyAsync(c->last_counts, c->compact.totals.p, nq * sizeof(uint64_t), cudaMemcpyDeviceToHost, s));
   FEI_CUDA(cudaEventRecord(c->ev[4], s));
@@ -1853,15 +1753,15 @@ int finish_timing(fei_corpus* c, bool compacted) {
   FEI_CUDA(cudaEventElapsedTime(&t, c->ev[0], c->ev[1])); c->timing.h2d_ms = t;
   FEI_CUDA(cudaEventElapsedTime(&t, c->ev[1], c->ev[2])); c->timing.head_ms = t;
   FEI_CUDA(cudaEventElapsedTime(&t, c->ev[2], c->ev[3])); c->timing.body_ms = t;
-  if (compacted) { FEI_CUDA(cudaEventElapsedTime(&t, c->ev[3], c->ev[4])); c->timing.compact_ms = t; }   // what is left after the last chunk's scan
+  if (compacted) { FEI_CUDA(cudaEventElapsedTime(&t, c->ev[3], c->ev[4])); c->timing.compact_ms = t; }   // what is left after the body kernel
   FEI_CUDA(cudaEventElapsedTime(&t, c->ev[4], c->ev[5])); c->timing.d2h_ms = t;
   FEI_CUDA(cudaEventElapsedTime(&t, c->ev[0], c->ev[5])); c->timing.total_ms = t;
-  unsigned long long cnt[6] = {0, 0, 0, 0, 0, 0};
+  unsigned long long cnt[kWorkCounters] = {0};
   FEI_CUDA(cudaMemcpy(cnt, c->work_counter.as<unsigned long long>(), sizeof(cnt), cudaMemcpyDeviceToHost));
   c->timing.body_bytes_touched = cnt[1];
   c->timing.body_bytes_read = cnt[3];
   if (c->timing.body_kernel == 2u && cnt[4] > c->n / kGatherDiv) c->timing.body_kernel = 1u;   // k_body_sticky took the dense case
-  if (cnt[5]) { set_error("pipelined scan: a wait for the scan kernel's finished windows timed out"); return FEI_E_CUDA; }
+  if (cnt[5]) { set_error("ordered hit lists: a wait in the look-back or for a window's offsets (help_tail) timed out"); return FEI_E_CUDA; }
   return FEI_OK;
 }
 
@@ -1878,8 +1778,8 @@ int compact_masks(const uint32_t* masks, uint64_t n, uint32_t nq, uint64_t globa
   FEI_TRY(sc.blk_offsets.ensure(nblocks * nq * sizeof(uint64_t)));
   FEI_TRY(sc.totals.ensure(32 * sizeof(uint64_t)));
   FEI_CUDA(cudaMemsetAsync(sc.totals.p, 0, 32 * sizeof(uint64_t), s));
-  k_count<<<(unsigned)nblocks, kCompactBlock, 0, s>>>(masks, n, nq, 0, sc.blk_counts.as<uint32_t>());
-  k_scan_blocks<<<nq, 256, 0, s>>>(sc.blk_counts.as<uint32_t>(), 0, nblocks, nq, sc.blk_offsets.as<uint64_t>(), sc.totals.as<uint64_t>());
+  k_count<<<(unsigned)nblocks, kCompactBlock, 0, s>>>(masks, n, nq, sc.blk_counts.as<uint32_t>());
+  k_scan_blocks<<<nq, 256, 0, s>>>(sc.blk_counts.as<uint32_t>(), nblocks, nq, sc.blk_offsets.as<uint64_t>(), sc.totals.as<uint64_t>());
   if (launches) *launches += 2;
   FEI_CUDA(cudaMemcpyAsync(counts_out, sc.totals.p, nq * sizeof(uint64_t), cudaMemcpyDeviceToHost, s));
   FEI_CUDA(cudaStreamSynchronize(s));
@@ -1888,7 +1788,7 @@ int compact_masks(const uint32_t* masks, uint64_t n, uint32_t nq, uint64_t globa
     for (uint32_t q = 0; q < nq; ++q) if (counts_out[q] > stride) stride = counts_out[q];
     if (stride_out) *stride_out = stride;
     FEI_TRY(lists->ensure(stride * nq * sizeof(uint64_t)));
-    k_emit<<<(unsigned)nblocks, kCompactBlock, 0, s>>>(masks, n, nq, sc.blk_offsets.as<uint64_t>(), 0, global_base, stride, lists->as<uint64_t>());
+    k_emit<<<(unsigned)nblocks, kCompactBlock, 0, s>>>(masks, n, nq, sc.blk_offsets.as<uint64_t>(), global_base, stride, lists->as<uint64_t>());
     if (launches) *launches += 1;
   }
   FEI_CUDA(cudaGetLastError());
@@ -1906,14 +1806,8 @@ int compact_segments(const uint32_t* masks, uint64_t seg_stride, const uint64_t*
   FEI_TRY(sc.blk_offsets.ensure((nb_max ? nb_max : 1) * nq * sizeof(uint64_t)));
   FEI_TRY(sc.totals.ensure(32 * sizeof(uint64_t)));
   FEI_CUDA(cudaMemsetAsync(sc.totals.p, 0, 32 * sizeof(uint64_t), s));
-  for (uint32_t r = 0; r < n_seg; ++r) {
-    const uint64_t n = seg_n[r], nb = (n + kCompactRecs - 1) / kCompactRecs;
-    if (!n) continue;
-    const uint32_t* m = masks + (size_t)r * seg_stride;
-    k_count<<<(unsigned)nb, kCompactBlock, 0, s>>>(m, n, nq, 0, sc.blk_counts.as<uint32_t>());
-    k_scan_blocks<<<nq, 256, 0, s>>>(sc.blk_counts.as<uint32_t>(), 0, nb, nq, sc.blk_offsets.as<uint64_t>(), sc.totals.as<uint64_t>());   // the carry runs on across segments
-    k_emit<<<(unsigned)nb, kCompactBlock, 0, s>>>(m, n, nq, sc.blk_offsets.as<uint64_t>(), 0, seg_base[r], stride, lists);
-  }
+  for (uint32_t r = 0; r < n_seg; ++r)                         // the totals run on across segments
+    if (seg_n[r]) compact_lists(masks + (size_t)r * seg_stride, seg_n[r], nq, seg_base[r], sc, stride, lists, s);
   if (totals_out) {
     FEI_CUDA(cudaMemcpyAsync(totals_out, sc.totals.p, nq * sizeof(uint64_t), cudaMemcpyDeviceToHost, s));
     FEI_CUDA(cudaStreamSynchronize(s));
@@ -1941,7 +1835,7 @@ using namespace fei;
 extern "C" int fei_scan_masks(fei_corpus* c, const uint8_t* prog, uint64_t prog_len, uint32_t* masks) {
   if (!c) { set_error("null corpus"); return FEI_E_BADARG; }
   std::lock_guard<std::mutex> lock(c->mu);
-  FEI_TRY(run_scan(c, prog, prog_len, kCompactNone, nullptr, 0));
+  FEI_TRY(run_scan(c, prog, prog_len, kCompactNone, nullptr));
   if (masks && c->n) FEI_CUDA(cudaMemcpyAsync(masks, c->hits.p, c->n * sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx().stream));
   return finish_timing(c, false);
 }
@@ -1949,7 +1843,7 @@ extern "C" int fei_scan_masks(fei_corpus* c, const uint8_t* prog, uint64_t prog_
 extern "C" int fei_scan_count(fei_corpus* c, const uint8_t* prog, uint64_t prog_len, uint64_t* nhits) {
   if (!c) { set_error("null corpus"); return FEI_E_BADARG; }
   std::lock_guard<std::mutex> lock(c->mu);
-  FEI_TRY(run_scan(c, prog, prog_len, kCompactLists, nullptr, 0));     // lists stay on the device (fei_comm_allgather_hits, fei_scan_list_checksum)
+  FEI_TRY(run_scan(c, prog, prog_len, kCompactLists, nullptr));     // lists stay on the device (fei_comm_allgather_hits, fei_scan_list_checksum)
   FEI_TRY(finish_timing(c, true));
   if (nhits) for (uint32_t q = 0; q < c->last_nq; ++q) nhits[q] = c->last_counts[q];
   return FEI_OK;
@@ -1960,7 +1854,7 @@ extern "C" int fei_scan_hits(fei_corpus* c, const uint8_t* prog, uint64_t prog_l
   if (!c) { set_error("null corpus"); return FEI_E_BADARG; }
   std::lock_guard<std::mutex> lock(c->mu);
   if (!hits || !cap || !nhits) { set_error("null argument"); return FEI_E_BADARG; }
-  FEI_TRY(run_scan(c, prog, prog_len, kCompactLists, nullptr, 0));
+  FEI_TRY(run_scan(c, prog, prog_len, kCompactLists, nullptr));
   cudaStream_t s = ctx().stream;
   FEI_CUDA(cudaStreamSynchronize(s));                                  // the counts decide how much of every list is copied
   bool truncated = false;
@@ -2092,7 +1986,7 @@ extern "C" int fei_corpus_token_histogram(fei_corpus* c, const uint8_t* prog, ui
   if (!c || !n_tokens || !tok_off) { set_error("null argument"); return FEI_E_BADARG; }
   std::lock_guard<std::mutex> lock(c->mu);
   *n_tokens = 0; tok_off[0] = 0;
-  FEI_TRY(run_scan(c, prog, prog_len, kCompactNone, nullptr, 0));
+  FEI_TRY(run_scan(c, prog, prog_len, kCompactNone, nullptr));
   fei_prog_hdr h; memcpy(&h, prog, sizeof(h));
   if (h.n_queries != 1 || h.n_slots < 1) { set_error("token histogram wants one query whose first header field names the column"); return FEI_E_BADARG; }
   if (c->n == 0) return finish_timing(c, false);

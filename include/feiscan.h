@@ -363,11 +363,11 @@ int fei_comm_bind_corpus(fei_corpus* c);
 int fei_comm_is_p2p(void);
 int fei_comm_last_exchange_in_kernel(void);   /* 1: the last fei_comm_scan_gather stored its masks into the peers from inside the scan kernel */
 /* Collective: the scan of fei_scan_count (masks + ordered local lists) with the hit all-gather
- * folded in: the scan runs in chunks, and the masks of a finished chunk are written into every
- * peer's buffer by copy-engine transfers (or a grouped ncclBroadcast) while the next chunk is
- * scanned.  On return every rank holds the masks of ALL shards, rank-major = global listing
- * order, and nhits_total[q] = global hits of query q.  The buffers are overwritten as soon as
- * any rank enters the next gather.                                                            */
+ * folded in: the scan kernel stores each finished window of masks into every peer's buffer while
+ * it scans the next ones (without peer memory, or with FEI_COMM_KERNEL_PUSH=0, copy-engine
+ * transfers or a grouped ncclBroadcast move the masks after the scan).  On return every rank
+ * holds the masks of ALL shards, rank-major = global listing order, and nhits_total[q] = global
+ * hits of query q.  The buffers are overwritten as soon as any rank enters the next gather.     */
 int fei_comm_scan_gather(fei_corpus* c, const uint8_t* prog, uint64_t prog_len, uint64_t* nhits_total);
 /* Lengths and order-sensitive checksums (see fei_scan_list_checksum) of the GLOBAL ordered hit
  * lists the last gather on this rank stands for (fei_comm_scan_gather / fei_comm_allgather_hits). */

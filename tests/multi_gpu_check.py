@@ -7,9 +7,9 @@ when the box has at least two GPUs):
 Every rank scans its record range; the results are exchanged through libfeiscan's multi-GPU paths and rank 0 compares the
 gathered GLOBAL ordered lists with the oracle on the whole corpus:
   * fei_comm_allgather_hits   : adaptive all-gatherv after a scan (sparse = grouped ncclBroadcast of the lists, dense = masks);
-  * fei_comm_scan_gather      : chunked scan with the mask all-gather of a finished chunk overlapped with the next chunk's scan
-                                (peer-memory copies over CUDA IPC, or grouped ncclBroadcast with FEI_COMM_P2P=0): totals,
-                                order-sensitive checksums and the materialised global lists;
+  * fei_comm_scan_gather      : scan with the mask all-gather folded in (peer stores from inside the scan kernel, peer-memory
+                                copies over CUDA IPC after the scan with FEI_COMM_KERNEL_PUSH=0, or a grouped ncclBroadcast
+                                with FEI_COMM_P2P=0): totals, order-sensitive checksums and the materialised global lists;
   * fei_comm_allreduce_first_bad : 8-byte min-reduce of a range-sharded chain."""
 import ctypes as C
 import os
@@ -83,11 +83,10 @@ def main():
                 assert (int(gt[q]),) + checksum(want[q]) == (len(want[q]), int(ga[q]), int(gs[q])), (name, p, "checksum")
             print(f"[multi_gpu_check] {name}: all-gatherv over {world} ranks ok ({[int(x) for x in tot[:nq]]} hits)", flush=True)
         dist.barrier()
-        # ---- the scan with the gather folded in, over peer memory and over NCCL, with several chunks
-        for p2p, push, chunks in (("1", "1", "3"), ("1", "1", "1"), ("1", "0", "3"), ("0", "1", "3")):
+        # ---- the scan with the gather folded in, over peer memory and over NCCL
+        for p2p, push in (("1", "1"), ("1", "0"), ("0", "1")):
             os.environ["FEI_COMM_P2P"] = p2p                 # peer memory (CUDA IPC) or NCCL
-            os.environ["FEI_COMM_KERNEL_PUSH"] = push        # peer stores from inside the scan kernel, or copy engines chunk by chunk
-            os.environ["FEI_SCAN_CHUNKS"] = chunks
+            os.environ["FEI_COMM_KERNEL_PUSH"] = push        # peer stores from inside the scan kernel, or copy engines after it
             _abi.check(lib.fei_comm_bind_corpus(corpus.handle))
             tot2 = np.zeros(32, dtype=np.uint64)
             _abi.check(lib.fei_comm_scan_gather(corpus.handle, prog, len(prog), _abi.ptr(tot2)))
@@ -101,23 +100,21 @@ def main():
                     assert checksum(want[q]) == (int(ga[q]), int(gs[q])), (name, p, "checksum of the gathered masks")
                     mine = [i for i in want[q] if a <= i < b]
                     assert checksum(mine) == (int(la[q]), int(ls[q])), (name, p, "local lists")
-                how = "NCCL" if not lib.fei_comm_is_p2p() else "peer stores inside the scan kernel" if lib.fei_comm_last_exchange_in_kernel() else "peer copies per chunk"
-                print(f"[multi_gpu_check] {name}: scan+gather ({how}, {chunks} chunk(s)) ok", flush=True)
+                how = "NCCL" if not lib.fei_comm_is_p2p() else "peer stores inside the scan kernel" if lib.fei_comm_last_exchange_in_kernel() else "peer copies after the scan"
+                print(f"[multi_gpu_check] {name}: scan+gather ({how}) ok", flush=True)
             if lib.fei_comm_is_p2p():
                 assert bool(lib.fei_comm_last_exchange_in_kernel()) == (push == "1"), "which path moved the masks"
             dist.barrier()
-        os.environ.pop("FEI_SCAN_CHUNKS"); os.environ.pop("FEI_COMM_P2P"); os.environ.pop("FEI_COMM_KERNEL_PUSH")
-    # a query with header predicates: the head pass runs first, the content pass is chunked
+        os.environ.pop("FEI_COMM_P2P"); os.environ.pop("FEI_COMM_KERNEL_PUSH")
+    # a query with header predicates: the head pass runs first, then the content pass
     pb = ProgramBuilder()
     pb.add_query([Cond(C_FLAGS, pattern=Pattern("exact_contains", "F")), Cond(C_BODY, pattern=Pattern("regex", "python|rust", re.IGNORECASE))])
     prog = pb.build()
-    os.environ["FEI_SCAN_CHUNKS"] = "2"
     _abi.check(lib.fei_comm_bind_corpus(corpus.handle))
     tot2 = np.zeros(32, dtype=np.uint64)
     _abi.check(lib.fei_comm_scan_gather(corpus.handle, prog, len(prog), _abi.ptr(tot2)))
     gt = np.zeros(32, dtype=np.uint64); ga = np.zeros(32, dtype=np.uint64); gs = np.zeros(32, dtype=np.uint64)
     _abi.check(lib.fei_comm_gathered_checksum(1, _abi.ptr(gt), _abi.ptr(ga), _abi.ptr(gs)))
-    os.environ.pop("FEI_SCAN_CHUNKS")
     if rank == 0:
         want = mo.run_search(mems, [{"field": "flags", "operator": "has_flag", "value": "F"}, {"field": "content", "operator": "matches", "value": "python|rust"}])
         assert (len(want),) + checksum(want) == (int(tot2[0]), int(ga[0]), int(gs[0])), "head + body scan+gather"

@@ -14,7 +14,6 @@ pytestmark = pytest.mark.gpu
 SEED = 0xB0D1
 BASE = 123_456_789
 SIZES = [1, 31, 4095, 4096, 4097, 3 * 4096 + 17, 80 * 4096 + 123]
-WAYS = [{}, {"FEI_SCAN_CHUNKS": "3"}, {"FEI_SCAN_CHUNKS": "3", "FEI_SCAN_CHUNK_LAUNCHES": "1"}]
 BODY = 3                                                           # fei_scan_timing.body_kernel of k_body
 
 BATCH32 = ["python", "docker|kubernetes", "neural networks", "react", "angular", "rust", "django", "flask", "terraform", "ansible",
@@ -74,46 +73,41 @@ def _checksums(lists):
     return a, s
 
 
-def _check(c, name, monkeypatch):
+def _check(c, name):
     prog, nq = _prog(name)
     expect = PROGRAMS[name][1]
-    for env in WAYS:
-        with monkeypatch.context() as mp:
-            for k, v in env.items():
-                mp.setenv(k, v)
-            masks = c.scan_masks(prog)
-            want = [np.nonzero((masks >> np.uint32(q)) & np.uint32(1))[0].astype(np.uint64) + np.uint64(BASE) for q in range(nq)]
-            got = c.scan_hits(prog, nq)                            # fei_scan_count, then fei_scan_fetch_hits
-            tm = c.timing()
-            assert tm["body_kernel"] == BODY, (env, tm)
-            if expect is not None:
-                assert tm["body_direct"] == expect[0], (env, tm)
-                if expect[1] is not None:
-                    assert tm["body_acc_mode"] == expect[1], (env, tm)
-                if not env:
-                    assert tm["kernel_launches"] == 1, tm          # body only: the lists need no kernel of their own
-            for q in range(nq):
-                assert np.array_equal(got[q], want[q]), (name, env, q, len(got[q]), len(want[q]))
-            a, s = c.list_checksums(nq)
-            wa, ws = _checksums(want)
-            assert [int(x) for x in a] == wa and [int(x) for x in s] == ws, (name, env)
-            got2 = c.scan_hits(prog, nq, cap=max(1, c.n))           # fei_scan_hits
-            for q in range(nq):
-                assert np.array_equal(got2[q], want[q]), (name, env, q)
+    masks = c.scan_masks(prog)
+    want = [np.nonzero((masks >> np.uint32(q)) & np.uint32(1))[0].astype(np.uint64) + np.uint64(BASE) for q in range(nq)]
+    got = c.scan_hits(prog, nq)                                    # fei_scan_count, then fei_scan_fetch_hits
+    tm = c.timing()
+    assert tm["body_kernel"] == BODY, tm
+    if expect is not None:
+        assert tm["body_direct"] == expect[0], tm
+        if expect[1] is not None:
+            assert tm["body_acc_mode"] == expect[1], tm
+        assert tm["kernel_launches"] == 1, tm                      # body only: the lists need no kernel of their own
+    for q in range(nq):
+        assert np.array_equal(got[q], want[q]), (name, q, len(got[q]), len(want[q]))
+    a, s = c.list_checksums(nq)
+    wa, ws = _checksums(want)
+    assert [int(x) for x in a] == wa and [int(x) for x in s] == ws, name
+    got2 = c.scan_hits(prog, nq, cap=max(1, c.n))                   # fei_scan_hits
+    for q in range(nq):
+        assert np.array_equal(got2[q], want[q]), (name, q)
     return want
 
 
 @pytest.mark.parametrize("name", list(PROGRAMS))
-def test_window_lists_equal_the_masks(corpus, name, monkeypatch):
-    want = _check(corpus, name, monkeypatch)
+def test_window_lists_equal_the_masks(corpus, name):
+    want = _check(corpus, name)
     if corpus.n >= 4096 and name != "class-indexed":
         assert any(len(w) for w in want)                           # not vacuous
 
 
-def test_two_programs_back_to_back(corpus, monkeypatch):
+def test_two_programs_back_to_back(corpus):
     """The descriptors and window counters of one scan are reset for the next, whatever its query count."""
-    want_a = _check(corpus, "batch32", monkeypatch)
-    _check(corpus, "acc1-negated-zero", monkeypatch)
+    want_a = _check(corpus, "batch32")
+    _check(corpus, "acc1-negated-zero")
     prog, nq = _prog("batch32")
     got = corpus.scan_hits(prog, nq)
     for q in range(nq):

@@ -254,14 +254,15 @@ def _explain(prog, ref, queries, want, got):
             f"CPU model of the serialized automaton gives content bits {m.run(ref.bodies[r]):#x}")
 
 
-def _scan_all_ways(c, ref, queries, expect, monkeypatch, head_fuse_too):
+def _scan_all_ways(c, ref, queries, expect, monkeypatch, head):
+    """head: the program has header conditions too, so it also runs with the unfused header pass."""
     prog = _program(queries)
     nq = len(queries)
     want = ref.masks(queries)
     want_lists = [np.nonzero(want >> np.uint32(q) & 1)[0].astype(np.uint64) for q in range(nq)]
-    ways = [{}, {"FEI_SCAN_CHUNKS": "3"}, {"FEI_SCAN_CHUNKS": "3", "FEI_SCAN_CHUNK_LAUNCHES": "1"}]
-    if head_fuse_too:
-        ways.append({"FEI_HEAD_FUSE": "0"})
+    ways = [{}, {"FEI_HEAD_FUSE": "0"}] if head else [{}]
+    # body only: one scan launch; k_body builds the ordered lists itself, k_body_sticky's are compacted by three kernels after it
+    launches = None if head else {BODY: 1, STICKY: 4}[expect[0]]
     for env in ways:
         with monkeypatch.context() as mp:
             for k, v in env.items():
@@ -273,7 +274,11 @@ def _scan_all_ways(c, ref, queries, expect, monkeypatch, head_fuse_too):
             assert np.array_equal(got, want), (env, _explain(prog, ref, queries, want, got))
             hits = c.scan_hits(prog, nq)
             assert _path(c.timing()) == expect
+            if launches is not None:
+                assert c.timing()["kernel_launches"] == launches, (env, c.timing())
             counts = c.scan_count(prog, nq)
+            if launches is not None:
+                assert c.timing()["kernel_launches"] == launches, (env, c.timing())
         for q in range(nq):
             assert np.array_equal(hits[q], want_lists[q]), (env, q)
             assert int(counts[q]) == want_lists[q].size, (env, q)
@@ -289,7 +294,7 @@ def test_content_paths_agree_with_cpython(corpus, name, monkeypatch):
         path = predicted_path(_program(queries))
         if expect is not None:
             assert path == expect, (name, path)
-        want = _scan_all_ways(c, ref, queries, path, monkeypatch, head_fuse_too=head)
+        want = _scan_all_ways(c, ref, queries, path, monkeypatch, head=head)
         assert want.any() and (want != want[0]).any()                  # the case is not vacuous
 
 
@@ -330,7 +335,7 @@ def test_gather_switch_over(gather_corpus, selected, kernel, monkeypatch):
     p = _rx(STICKY_PAT)
     g = f"g{selected}"
     queries = [[_tag(g), _bc(p)], [_tag(g), _bc(p, negate=True)], [_bc(p), _tag(g), _tag("misc")]]
-    want = _scan_all_ways(c, ref, queries, (kernel, 1, 3), monkeypatch, head_fuse_too=True)
+    want = _scan_all_ways(c, ref, queries, (kernel, 1, 3), monkeypatch, head=True)
     if selected:
         assert (want & 1).any() and (selected == 1 or (want & 2).any())
     else:

@@ -28,7 +28,7 @@ Counts per kernel of the mnemonics that show the design: UBLKCP.S.G = cp.async.b
 arrive / expect_tx / try_wait, ELECT = elected issuing lane, VOTE* = warp ballots, SHFL = warp shuffles, LDS.U16 = one automaton lookup
 per byte, LDS.128 = ring read-back, LDG.E.NA.128.CONSTANT = ld.global.nc.L1::no_allocate.v4 streaming loads, LDG/STG.E.128 = 16-byte
 rows, ATOMG / REDG = global atomics (work counters, window completion counters, hit counts), SHF.R.W = 32-bit rotates (SHA-256),
-NANOSLEEP = the gate kernel's back-off, D* = FP64 (only the shortest-repr float formatter's checks), no MATCH anywhere.
+NANOSLEEP = the back-off of the ordered-list look-back and help_tail waits, D* = FP64 (only the shortest-repr float formatter's checks), no MATCH anywhere.
 """)
 for (name, c), dm in sorted(zip(counts.items(), demangle), key=lambda t: t[1]):
     short = re.sub(r"\(.*", "", dm)
