@@ -574,6 +574,20 @@ __device__ __forceinline__ uint4 ldg_stream16(const void* p) {
   asm volatile("ld.global.nc.L1::no_allocate.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w) : "l"(p));
   return r;
 }
+// Stage a content automaton into shared memory with TMA bulk copies (cp.async.bulk + mbarrier), at most 32 KiB per copy.
+// Its __syncthreads also publishes to the CTA what any thread wrote to shared memory before the call.
+__device__ __forceinline__ void stage_table(uint8_t* dst, const uint8_t* src, uint32_t bytes, uint64_t* bar) {
+  if (threadIdx.x == 0) { mbar_init(bar, 1); asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    mbar_expect_tx(bar, bytes);
+    for (uint32_t o = 0; o < bytes; o += 32768u) {
+      uint32_t nb = bytes - o < 32768u ? bytes - o : 32768u;
+      bulk_g2s(dst + o, src + o, nb, bar);
+    }
+  }
+  mbar_wait(bar, 0);
+}
 
 struct BodyArgs {
   const uint8_t* prog;
@@ -905,6 +919,23 @@ struct BodyDecide {
   }
 };
 
+// The hit mask of a record whose content verdict is acc: of the queries in `alive`, those whose every content condition
+// holds (bit `bit` of acc, inverted when negated).  Conditions of the other kinds are already settled in `alive`.
+__device__ __forceinline__ uint32_t content_hits(uint32_t acc, uint32_t alive, const fei_prog_query* queries,
+                                                 const fei_prog_cond* conds, uint32_t nq) {
+  uint32_t hit = 0;
+  for (uint32_t q = 0; q < nq; ++q) {
+    if (!(alive >> q & 1)) continue;
+    bool ok = true;
+    for (uint32_t c = queries[q].cond_begin; ok && c < queries[q].cond_end; ++c) {
+      const fei_prog_cond& cd = conds[c];
+      if (cd.kind == FEI_C_BODY) ok = ((acc >> cd.bit) & 1u) != cd.negate;
+    }
+    if (ok) hit |= 1u << q;
+  }
+  return hit;
+}
+
 template <bool kDirect, int kAcc, bool kPush>
 __global__ void __launch_bounds__(kBodyThreads, 1) k_body(BodyArgs a) {
   extern __shared__ __align__(128) uint8_t smem[];
@@ -916,6 +947,7 @@ __global__ void __launch_bounds__(kBodyThreads, 1) k_body(BodyArgs a) {
   const fei_prog_cond* conds = reinterpret_cast<const fei_prog_cond*>(a.prog + ph->off_conds);
   const fei_prog_query* queries = reinterpret_cast<const fei_prog_query*>(a.prog + ph->off_queries);
   const uint32_t nq = ph->n_queries;
+  // written by warp 0 before stage_table, whose __syncthreads publishes it to the other warps
   if (kAcc != 3 && threadIdx.x < 32) {
     uint32_t bits = 0;
     if (threadIdx.x < nq)
@@ -925,18 +957,7 @@ __global__ void __launch_bounds__(kBodyThreads, 1) k_body(BodyArgs a) {
     bits = __reduce_or_sync(0xffffffffu, bits);
     if (threadIdx.x == 0) q_need[32] = bits;
   }
-  // ---- stage the automaton into shared memory with TMA bulk copies (cp.async.bulk + mbarrier)
-  if (threadIdx.x == 0) { mbar_init(&bar, 1); asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    mbar_expect_tx(&bar, table_bytes);
-    const uint8_t* src = a.prog + dd->off_trans;
-    for (uint32_t o = 0; o < table_bytes; o += 32768u) {
-      uint32_t nb = table_bytes - o < 32768u ? table_bytes - o : 32768u;
-      bulk_g2s(smem + o, src + o, nb, &bar);
-    }
-  }
-  mbar_wait(&bar, 0);
+  stage_table(smem, a.prog + dd->off_trans, table_bytes, &bar);
   const uint32_t* endout = reinterpret_cast<const uint32_t*>(smem + (dd->off_endout - dd->off_trans));
   const uint32_t start = dd->start;
   const uint32_t all_q = nq >= 32 ? 0xFFFFFFFFu : ((1u << nq) - 1u);
@@ -1009,18 +1030,7 @@ __global__ void __launch_bounds__(kBodyThreads, 1) k_body(BodyArgs a) {
       if (__ballot_sync(0xffffffffu, k1 < lim) == 0) break;
     }
     if (live) {
-      const uint32_t acc = d.finish(endout);
-      uint32_t hit = 0;
-      for (uint32_t q = 0; q < nq; ++q) {
-        if (!(alive >> q & 1)) continue;
-        bool ok = true;
-        for (uint32_t c = queries[q].cond_begin; ok && c < queries[q].cond_end; ++c) {
-          const fei_prog_cond& cd = conds[c];
-          if (cd.kind == FEI_C_BODY) ok = ((acc >> cd.bit) & 1u) != cd.negate;
-        }
-        if (ok) hit |= 1u << q;
-      }
-      a.hits[rec] = hit;
+      a.hits[rec] = content_hits(d.finish(endout), alive, queries, conds, nq);
     } else if (rec != kInvalidRec && !a.has_alive) {
       a.hits[rec] = 0;
     }
@@ -1075,6 +1085,16 @@ constexpr unsigned long long kGatherDiv = 16;       // k_body_gather takes over 
 constexpr uint32_t kStickyAddrLimit = 65535u;
 constexpr uint32_t kStickyAddrSlack = 4096u;     // head-room the host leaves for the shared-memory window base
 
+// Rewrite the staged transitions at smem (shared address trans_s) in place from state index to row address
+// (trans_s + state * stride2), for k_body_sticky and k_body_gather.
+__device__ __forceinline__ void rows_to_addresses(uint8_t* smem, const fei_prog_dfa* dd, uint32_t trans_s, uint32_t stride2) {
+  if (trans_s + dd->n_states * stride2 > kStickyAddrLimit) __trap();      // host-side eligibility test left 4 KiB of slack
+  uint16_t* t = reinterpret_cast<uint16_t*>(smem);
+  const uint32_t n_entries = dd->n_states * dd->row_stride;
+  for (uint32_t i = threadIdx.x; i < n_entries; i += kBodyThreads) t[i] = (uint16_t)(trans_s + (uint32_t)t[i] * stride2);
+  __syncthreads();
+}
+
 template <bool kPush>
 __global__ void __launch_bounds__(kBodyThreads, 1) k_body_sticky(BodyArgs a) {
   extern __shared__ __align__(128) uint8_t smem[];
@@ -1083,18 +1103,8 @@ __global__ void __launch_bounds__(kBodyThreads, 1) k_body_sticky(BodyArgs a) {
   const fei_prog_hdr* ph = reinterpret_cast<const fei_prog_hdr*>(a.prog);
   const fei_prog_dfa* dd = reinterpret_cast<const fei_prog_dfa*>(a.prog + ph->off_body_dfa);
   const uint32_t table_bytes = dd->table_bytes;
-  if (threadIdx.x == 0) { mbar_init(&bar, 1); asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    mbar_expect_tx(&bar, table_bytes);
-    const uint8_t* src = a.prog + dd->off_trans;
-    for (uint32_t o = 0; o < table_bytes; o += 32768u) {
-      uint32_t nb = table_bytes - o < 32768u ? table_bytes - o : 32768u;
-      bulk_g2s(smem + o, src + o, nb, &bar);
-    }
-  }
-  mbar_wait(&bar, 0);
-  const uint32_t trans_s = smem_u32(smem), stride2 = dd->row_stride * 2u, n_entries = dd->n_states * dd->row_stride;
+  stage_table(smem, a.prog + dd->off_trans, table_bytes, &bar);
+  const uint32_t trans_s = smem_u32(smem), stride2 = dd->row_stride * 2u;
   // per-warp ring + its mbarriers, behind the table
   const uint32_t warp = threadIdx.x >> 5;
   uint8_t* ring = smem + ((table_bytes + 127u) & ~127u) + warp * kWarpRingBytes;
@@ -1103,12 +1113,7 @@ __global__ void __launch_bounds__(kBodyThreads, 1) k_body_sticky(BodyArgs a) {
   if ((threadIdx.x & 31) < kStages) mbar_init(&bars[threadIdx.x & 31], 1);
   asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   uint32_t prod = 0, cons = 0;                       // chunks issued / consumed by this warp since kernel start (stage = count % kStages)
-  if (trans_s + dd->n_states * stride2 > kStickyAddrLimit) __trap();      // host-side eligibility test left 4 KiB of slack
-  {
-    uint16_t* t = reinterpret_cast<uint16_t*>(smem);
-    for (uint32_t i = threadIdx.x; i < n_entries; i += kBodyThreads) t[i] = (uint16_t)(trans_s + (uint32_t)t[i] * stride2);
-  }
-  __syncthreads();
+  rows_to_addresses(smem, dd, trans_s, stride2);
   const uint32_t* endout = reinterpret_cast<const uint32_t*>(smem + (dd->off_endout - dd->off_trans));
   const uint32_t start_e = trans_s + dd->start * stride2;
   const uint32_t sticky_e = dd->sticky != 0xFFFFFFFFu ? trans_s + (dd->sticky - 1u) * stride2 : 0xFFFFFFFFu;
@@ -1282,18 +1287,7 @@ __global__ void __launch_bounds__(kBodyThreads, 1) k_body_sticky(BodyArgs a) {
   };
   auto close_group = [&](const Grp& G) {
     if (G.live) {
-      const uint32_t acc = endout[(G.e - trans_s) / stride2];
-      uint32_t hit = 0;
-      for (uint32_t q = 0; q < nq; ++q) {
-        if (!(G.alive >> q & 1)) continue;
-        bool ok = true;
-        for (uint32_t c = queries[q].cond_begin; ok && c < queries[q].cond_end; ++c) {
-          const fei_prog_cond& cd = conds[c];
-          if (cd.kind == FEI_C_BODY) ok = ((acc >> cd.bit) & 1u) != cd.negate;
-        }
-        if (ok) hit |= 1u << q;
-      }
-      a.hits[G.rec] = hit;
+      a.hits[G.rec] = content_hits(endout[(G.e - trans_s) / stride2], G.alive, queries, conds, nq);
     } else if (G.rec != kInvalidRec && !a.has_alive) {
       a.hits[G.rec] = 0;
     }
@@ -1349,25 +1343,9 @@ __global__ void __launch_bounds__(kBodyThreads, 1) k_body_gather(BodyArgs a, con
   if (n_live == 0 || n_live > a.gather_max) return;            // k_body_sticky takes the dense case (uniform for the grid)
   const fei_prog_hdr* ph = reinterpret_cast<const fei_prog_hdr*>(a.prog);
   const fei_prog_dfa* dd = reinterpret_cast<const fei_prog_dfa*>(a.prog + ph->off_body_dfa);
-  const uint32_t table_bytes = dd->table_bytes;
-  if (threadIdx.x == 0) { mbar_init(&bar, 1); asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    mbar_expect_tx(&bar, table_bytes);
-    const uint8_t* src = a.prog + dd->off_trans;
-    for (uint32_t o = 0; o < table_bytes; o += 32768u) {
-      uint32_t nb = table_bytes - o < 32768u ? table_bytes - o : 32768u;
-      bulk_g2s(smem + o, src + o, nb, &bar);
-    }
-  }
-  mbar_wait(&bar, 0);
-  const uint32_t trans_s = smem_u32(smem), stride2 = dd->row_stride * 2u, n_entries = dd->n_states * dd->row_stride;
-  if (trans_s + dd->n_states * stride2 > kStickyAddrLimit) __trap();
-  {
-    uint16_t* t = reinterpret_cast<uint16_t*>(smem);
-    for (uint32_t i = threadIdx.x; i < n_entries; i += kBodyThreads) t[i] = (uint16_t)(trans_s + (uint32_t)t[i] * stride2);
-  }
-  __syncthreads();
+  stage_table(smem, a.prog + dd->off_trans, dd->table_bytes, &bar);
+  const uint32_t trans_s = smem_u32(smem), stride2 = dd->row_stride * 2u;
+  rows_to_addresses(smem, dd, trans_s, stride2);
   const uint32_t* endout = reinterpret_cast<const uint32_t*>(smem + (dd->off_endout - dd->off_trans));
   const uint32_t start_e = trans_s + dd->start * stride2;
   const uint32_t sticky_e = dd->sticky != 0xFFFFFFFFu ? trans_s + (dd->sticky - 1u) * stride2 : 0xFFFFFFFFu;
@@ -1397,32 +1375,29 @@ __global__ void __launch_bounds__(kBodyThreads, 1) k_body_gather(BodyArgs a, con
       bytes_read += 16;
       if (e == sticky_e) break;                                  // matched: the verdict cannot change any more
     }
-    const uint32_t acc = endout[(e - trans_s) / stride2];
-    uint32_t hit = 0;
-    for (uint32_t q = 0; q < nq; ++q) {
-      if (!(alive >> q & 1)) continue;
-      bool ok = true;
-      for (uint32_t c = queries[q].cond_begin; ok && c < queries[q].cond_end; ++c) {
-        const fei_prog_cond& cd = conds[c];
-        if (cd.kind == FEI_C_BODY) ok = ((acc >> cd.bit) & 1u) != cd.negate;
-      }
-      if (ok) hit |= 1u << q;
-    }
-    a.hits[rec] = hit;
+    a.hits[rec] = content_hits(endout[(e - trans_s) / stride2], alive, queries, conds, nq);
   }
   for (int o = 16; o; o >>= 1) bytes_read += __shfl_down_sync(0xffffffffu, bytes_read, o);
   if ((threadIdx.x & 31) == 0 && bytes_read) { atomicAdd(a.counter + 3, bytes_read); atomicAdd(a.counter + 1, bytes_read); }
 }
 
-template <bool kDirect, int kAcc>
-static int launch_body(const BodyArgs& a, unsigned grid, size_t smem, cudaStream_t s) {
-  if (a.push_n) {
-    FEI_CUDA(cudaFuncSetAttribute(k_body<kDirect, kAcc, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    k_body<kDirect, kAcc, true><<<grid, kBodyThreads, smem, s>>>(a);
-  } else {
-    FEI_CUDA(cudaFuncSetAttribute(k_body<kDirect, kAcc, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    k_body<kDirect, kAcc, false><<<grid, kBodyThreads, smem, s>>>(a);
-  }
+// The content kernel of one scan: k_body_sticky when the sticky automaton's row addresses fit 16 bits, else the k_body
+// instance for the table's column mapping and accumulator mode.
+using BodyKernel = void (*)(BodyArgs);
+static BodyKernel body_kernel(bool sticky, bool direct, int acc_mode, bool push) {
+  static const BodyKernel k_body_of[2][2][4] = {      // [push][direct][acc_mode]
+      {{k_body<false, 0, false>, k_body<false, 1, false>, k_body<false, 2, false>, k_body<false, 3, false>},
+       {k_body<true, 0, false>, k_body<true, 1, false>, k_body<true, 2, false>, k_body<true, 3, false>}},
+      {{k_body<false, 0, true>, k_body<false, 1, true>, k_body<false, 2, true>, k_body<false, 3, true>},
+       {k_body<true, 0, true>, k_body<true, 1, true>, k_body<true, 2, true>, k_body<true, 3, true>}}};
+  if (sticky) return push ? k_body_sticky<true> : k_body_sticky<false>;
+  return k_body_of[push][direct][acc_mode];
+}
+
+template <typename Kernel, typename... Args>
+static int launch_body(Kernel k, unsigned grid, size_t smem, cudaStream_t s, Args... args) {
+  FEI_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  k<<<grid, kBodyThreads, smem, s>>>(args...);
   return FEI_OK;
 }
 
@@ -1698,8 +1673,7 @@ int run_scan(fei_corpus* c, const uint8_t* prog, uint64_t prog_len, int compact_
     a.gather_max = n / kGatherDiv;
     FEI_TRY(c->live_list.ensure((a.gather_max + 1) * sizeof(uint32_t)));
     k_live_list<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(c->hits.as<uint32_t>(), n, c->live_list.as<uint32_t>(), a.counter + 4, a.gather_max);
-    FEI_CUDA(cudaFuncSetAttribute(k_body_gather, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    k_body_gather<<<grid, kBodyThreads, smem, s>>>(a, c->live_list.as<uint32_t>(), c->rec_pos.as<uint32_t>());
+    FEI_TRY(launch_body(k_body_gather, grid, smem, s, a, c->live_list.as<uint32_t>(), c->rec_pos.as<uint32_t>()));
     launches += 2;
   }
   if (body_lists || push) {                                    // window counters (and, for body_lists, descriptors) for the scan
@@ -1716,19 +1690,8 @@ int run_scan(fei_corpus* c, const uint8_t* prog, uint64_t prog_len, int compact_
   }
   if (push) { a.push_peers = hook->push_peers; a.push_n = hook->push_n; a.push_off = hook->push_off; hook->pushed = true; }
   if (n && need_body) {
-    int rc = FEI_OK;
-    if (sticky_kernel) {
-      const size_t smem_sticky = ((smem + 127) & ~(size_t)127) + kStickyRingBytes;
-      if (a.push_n) {
-        FEI_CUDA(cudaFuncSetAttribute(k_body_sticky<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_sticky));
-        k_body_sticky<true><<<grid, kBodyThreads, smem_sticky, s>>>(a);
-      } else {
-        FEI_CUDA(cudaFuncSetAttribute(k_body_sticky<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_sticky));
-        k_body_sticky<false><<<grid, kBodyThreads, smem_sticky, s>>>(a);
-      }
-    } else if (direct) rc = acc_mode == 3 ? launch_body<true, 3>(a, grid, smem, s) : acc_mode == 1 ? launch_body<true, 1>(a, grid, smem, s) : acc_mode == 2 ? launch_body<true, 2>(a, grid, smem, s) : launch_body<true, 0>(a, grid, smem, s);
-    else rc = acc_mode == 3 ? launch_body<false, 3>(a, grid, smem, s) : acc_mode == 1 ? launch_body<false, 1>(a, grid, smem, s) : acc_mode == 2 ? launch_body<false, 2>(a, grid, smem, s) : launch_body<false, 0>(a, grid, smem, s);
-    FEI_TRY(rc);
+    const size_t body_smem = sticky_kernel ? ((smem + 127) & ~(size_t)127) + kStickyRingBytes : smem;   // k_body_sticky: + its rings
+    FEI_TRY(launch_body(body_kernel(sticky_kernel, direct, acc_mode, a.push_n != 0), grid, body_smem, s, a));
     ++launches;
   }
   FEI_CUDA(cudaEventRecord(c->ev[3], s));
