@@ -34,6 +34,11 @@ constexpr uint32_t kMaxCols = 8;           // header value columns kept per corp
 constexpr uint32_t kColUnits = 4;          // 16-byte units per column value (longer values: directory walk)
 constexpr uint16_t kColAbsent = 0xFFFF, kColWalk = 0xFFFE;
 constexpr uint32_t kInvalidRec = 0xFFFFFFFFu;
+#ifdef __CUDACC__
+// a record whose header the directory cannot address (hdir.cu) has the single entry {~0, ~0}: its header is parsed from the text
+__host__ __device__ __forceinline__ uint2 text_record_entry() { return make_uint2(0xFFFFFFFFu, 0xFFFFFFFFu); }
+__host__ __device__ __forceinline__ bool text_record(const uint2* ent, uint32_t n_ent) { return n_ent == 1 && ent[0].x == 0xFFFFFFFFu; }
+#endif
 #define FEI_MAX_AUX 4
 }
 

@@ -2,7 +2,7 @@
 // for every record, one entry per header line that holds a colon, in line order -- the dict that utils.py:113-118
 // builds (`for line in header.split("\n"): if ":" in line: key, value = line.split(":", 1);
 // headers[key.strip()] = value.strip()`), minus the dict's collapsing of repeated keys, which depends on the queried
-// field and stays in the scan (head_finish).  Keys are interned: the corpus keeps a dictionary of its distinct
+// field and stays in the scan (header_lookup in scan.cu).  Keys are interned: the corpus keeps a dictionary of its distinct
 // stripped key spellings (a few dozen in a real Memdir) and an entry names its key by dictionary slot, so a scan
 // runs the key automaton once per distinct key (k_key_lut) instead of once per header line of every record, and then
 // touches only the one value it needs.
@@ -14,7 +14,7 @@
 namespace fei {
 
 // entry.x = key slot | val_len << 16, entry.y = val_off (offset of the stripped value from the start of the record's
-// header text).  Headers longer than 65535 bytes get the single entry {~0, ~0}: "parse the text".
+// header text).  Headers longer than 65535 bytes get the single entry text_record_entry(): "parse the text".
 __device__ __forceinline__ unsigned long long key_hash(const uint8_t* p, uint32_t n) {
   unsigned long long h = 0xcbf29ce484222325ull;                       // FNV-1a, then a finaliser
   for (uint32_t i = 0; i < n; ++i) { h ^= p[i]; h *= 0x100000001b3ull; }
@@ -52,39 +52,32 @@ __global__ void __launch_bounds__(256) k_hdir(const uint8_t* __restrict__ hdr, c
   const uint64_t hlen = hdr_off[i + 1] - hdr_off[i];
   uint2* out = kPass ? dir + dir_off[i] : nullptr;
   if (hlen > 65535 || force_text) {
-    if (kPass) out[0] = make_uint2(0xFFFFFFFFu, 0xFFFFFFFFu); else { cnt[i] = 1; kd.cnt[kKeySlots] = 1u; }   // [kKeySlots]: some record's keys are not in the dictionary
+    if (kPass) out[0] = text_record_entry(); else { cnt[i] = 1; kd.cnt[kKeySlots] = 1u; }   // [kKeySlots]: some record's keys are not in the dictionary
     return;
   }
   uint32_t k = 0;
-  const uint8_t* hend = h + hlen;
-  const uint8_t* p = h;
-  while (p < hend) {
-    const uint8_t* eol = p; const uint8_t* colon = nullptr;
-    while (eol < hend && *eol != '\n') { if (!colon && *eol == ':') colon = eol; ++eol; }
-    if (colon) {
-      const uint8_t* ka = p; const uint8_t* kb = colon; strip_span(ka, kb);
-      const uint32_t klen = (uint32_t)(kb - ka);
-      const unsigned long long kh = key_hash(ka, klen);
-      if (!kPass) {
-        const uint32_t s = key_slot(kd, kh, true);
-        if (s == 0xFFFFFFFFu) atomicOr(kd.flag, 1u);
-        else {
-          const unsigned long long at = (unsigned long long)(ka - hdr);
-          if (at < kd.rep[s]) atomicMin(kd.rep + s, at);                 // representative = smallest offset; the plain read skips almost every atomic
-          kd.len[s] = klen;                                              // same hash => same length unless colliding (checked in pass 1)
-          if ((i & 63) == 0) atomicAdd(kd.cnt + s, 1u);                             // sampled frequency: which keys deserve a value column
-        }
-      } else {
-        const uint32_t s = key_slot(kd, kh, false);
-        bool same = s != 0xFFFFFFFFu && kd.len[s] == klen;
-        if (same) { const uint8_t* r = hdr + kd.rep[s]; for (uint32_t b = 0; same && b < klen; ++b) same = r[b] == ka[b]; }
-        if (!same) atomicOr(kd.flag, 2u);
-        const uint8_t* va = colon + 1; const uint8_t* vb = eol; strip_span(va, vb);
-        out[k] = make_uint2((s & 0xFFFFu) | (uint32_t)(vb - va) << 16, (uint32_t)(va - h));
+  HeaderLine l;
+  for (const uint8_t* p = h; p < h + hlen;) {
+    if (!next_header_line(p, h + hlen, l)) continue;
+    const uint32_t klen = (uint32_t)(l.kb - l.ka);
+    const unsigned long long kh = key_hash(l.ka, klen);
+    if (!kPass) {
+      const uint32_t s = key_slot(kd, kh, true);
+      if (s == 0xFFFFFFFFu) atomicOr(kd.flag, 1u);
+      else {
+        const unsigned long long at = (unsigned long long)(l.ka - hdr);
+        if (at < kd.rep[s]) atomicMin(kd.rep + s, at);                   // representative = smallest offset; the plain read skips almost every atomic
+        kd.len[s] = klen;                                                // same hash => same length unless colliding (checked in pass 1)
+        if ((i & 63) == 0) atomicAdd(kd.cnt + s, 1u);                    // sampled frequency: which keys deserve a value column
       }
-      ++k;
+    } else {
+      const uint32_t s = key_slot(kd, kh, false);
+      bool same = s != 0xFFFFFFFFu && kd.len[s] == klen;
+      if (same) { const uint8_t* r = hdr + kd.rep[s]; for (uint32_t b = 0; same && b < klen; ++b) same = r[b] == l.ka[b]; }
+      if (!same) atomicOr(kd.flag, 2u);
+      out[k] = make_uint2((s & 0xFFFFu) | (uint32_t)(l.vb - l.va) << 16, (uint32_t)(l.va - h));
     }
-    p = eol + 1;
+    ++k;
   }
   if (!kPass) cnt[i] = k;
 }
@@ -108,7 +101,7 @@ __global__ void __launch_bounds__(256) k_hdir_cols(const uint8_t* __restrict__ h
   if (i >= n) return;
   const uint2* ent = dir + dir_off[i];
   const uint32_t n_ent = (uint32_t)(dir_off[i + 1] - dir_off[i]);
-  if (n_ent == 1 && ent[0].x == 0xFFFFFFFFu) {                          // "parse the text" record: every column defers to the walk
+  if (text_record(ent, n_ent)) {                                        // every column defers to the walk
     for (uint32_t c = 0; c < n_cols; ++c) col_len[(uint64_t)c * n + i] = kColWalk;
     return;
   }

@@ -34,5 +34,18 @@ __device__ __forceinline__ void strip_span(const uint8_t*& a, const uint8_t*& b)
   for (;;) { if (a >= b) return; int n = ws_len_before(a, b); if (!n) break; b -= n; }
 }
 
+// One line of a header text, as utils.py:113-118 splits it: advances p past the line and its '\n'; false for a line without a
+// colon, else the key (before the first colon) and the value, both stripped.
+struct HeaderLine { const uint8_t *ka, *kb, *va, *vb; };
+__device__ __forceinline__ bool next_header_line(const uint8_t*& p, const uint8_t* end, HeaderLine& l) {
+  const uint8_t* eol = p; const uint8_t* colon = nullptr;
+  while (eol < end && *eol != '\n') { if (!colon && *eol == ':') colon = eol; ++eol; }
+  const uint8_t* line = p;
+  p = eol + 1;
+  if (!colon) return false;
+  l = HeaderLine{line, colon, colon + 1, eol};
+  strip_span(l.ka, l.kb); strip_span(l.va, l.vb);
+  return true;
+}
 
 }  // namespace fei

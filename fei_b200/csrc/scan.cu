@@ -8,11 +8,11 @@
 //
 // k_head_meta / k_head_parse : meta predicates (flags / date / folder / status) over the 20-byte meta columns, four
 //          records per thread; records that still need a header or name field go to a work list and get one thread
-//          each in k_head_parse, which reads the record's header directory (hdir.cu: interned key + stripped value
-//          span per header line; k_key_lut maps the corpus' distinct keys to the program's fields once per scan)
-//          and applies the reference's dict semantics (a repeated key keeps its last value, a case-insensitive
-//          field lookup takes the first matching spelling).  Headers the directory cannot address are split / stripped
-//          here exactly like utils.py:113-118.  Every string condition is an output bit of a byte DFA; the program
+//          each in k_head_parse, which applies the reference's dict semantics (header_lookup: a repeated key keeps its
+//          last value, a case-insensitive field lookup takes the first matching spelling) to the record's header lines:
+//          its header directory (hdir.cu: interned key + stripped value span per line; k_key_lut maps the corpus'
+//          distinct keys to the program's fields once per scan), or, for headers the directory cannot address, its
+//          text split / stripped like utils.py:113-118.  Every string condition is an output bit of a byte DFA; the program
 //          head (conditions + small automata) is staged into shared memory by a TMA bulk copy per CTA.
 //          Writes alive[i] = bitmask of queries whose non-content conditions all hold.
 // k_body : one warp per group of 32 records in the warp-transposed body tiles (corpus.h): each
@@ -36,113 +36,163 @@
 
 namespace fei {
 
-// ---------------------------------------------------------------- DFA view
-struct DfaView {
-  const uint16_t* trans;
-  const uint32_t* out;
-  const uint32_t* endout;
-  const uint8_t* cls;
-  uint32_t n_cols, stride, start, n_acc, empty_acc;
-};
-
-__device__ __forceinline__ DfaView dfa_view(const uint8_t* blob, uint32_t off) {
-  const fei_prog_dfa* d = reinterpret_cast<const fei_prog_dfa*>(blob + off);
-  DfaView v;
-  v.trans = reinterpret_cast<const uint16_t*>(blob + d->off_trans);
-  v.out = reinterpret_cast<const uint32_t*>(blob + d->off_out);
-  v.endout = reinterpret_cast<const uint32_t*>(blob + d->off_endout);
-  v.cls = blob + d->off_cls;
-  v.n_cols = d->n_cols; v.stride = d->row_stride; v.start = d->start; v.n_acc = d->n_acc; v.empty_acc = d->empty_acc;
-  return v;
-}
-
-// generic run over a byte span (tables in global memory or, for the head kernels, in the shared-memory copy of the
-// program head: plain loads, the address space is resolved at run time); used on short fields
-__device__ uint32_t dfa_run(const DfaView& d, const uint8_t* p, uint32_t len) {
-  if (len == 0) return d.empty_acc;
-  uint32_t s = d.start;
-  uint32_t acc = s < d.n_acc ? d.out[s] : 0u;
-  const bool direct = d.n_cols == 256;
-  for (uint32_t i = 0; i < len; ++i) {
-    uint32_t b = p[i];
-    uint32_t col = direct ? b : d.cls[b];
-    s = d.trans[s * d.stride + col];
-    if (s < d.n_acc) acc |= d.out[s];
-  }
-  return acc | d.endout[s];
-}
-
-// The same run with the tables in the shared-memory copy of the program head (stage_prog_head): 32-bit shared
-// addresses and ld.shared instead of generic 64-bit pointer arithmetic (the generic loop costs 29 instructions per
-// byte in SASS, this one about 8).
-struct DfaViewS { uint32_t trans, out, endout, cls, n_cols, stride2, start, n_acc, empty_acc; };
+// ---------------------------------------------------------------- short automaton runs (header fields, names, flags)
+// Where an automaton's tables live.  SmemTables: the shared-memory copy of the program head (stage_prog_head), 32-bit shared
+// addresses and ld.shared (a generic-pointer loop costs 29 instructions per byte in SASS, this one about 8).  GlobalTables: the
+// program blob in global memory.
 __device__ __forceinline__ uint32_t lds_u8(uint32_t a) { uint32_t r; asm volatile("ld.shared.u8 %0, [%1];" : "=r"(r) : "r"(a)); return r; }
 __device__ __forceinline__ uint32_t lds_u16(uint32_t a) { uint32_t r; asm volatile("ld.shared.u16 %0, [%1];" : "=r"(r) : "r"(a)); return r; }
 __device__ __forceinline__ uint32_t lds_u32(uint32_t a) { uint32_t r; asm volatile("ld.shared.u32 %0, [%1];" : "=r"(r) : "r"(a)); return r; }
-__device__ __forceinline__ DfaViewS dfa_view_s(const uint8_t* sblob, uint32_t off) {
-  const fei_prog_dfa* d = reinterpret_cast<const fei_prog_dfa*>(sblob + off);
-  const uint32_t base = (uint32_t)__cvta_generic_to_shared(sblob);
-  return DfaViewS{base + d->off_trans, base + d->off_out, base + d->off_endout, base + d->off_cls, d->n_cols, d->row_stride * 2u, d->start, d->n_acc, d->empty_acc};
-}
-// One automaton over a byte span in global memory.  out[] has an entry (0) for non-accepting states too, so there is no
-// branch around the lookup and the byte loads of an unrolled group issue ahead of the table walk.  (Fetching the span as
-// aligned 4- or 16-byte words was measured slower on the header workloads: per-lane skip / tail predicates diverge.)
-struct DfaStepS {
-  const DfaViewS& d; uint32_t s, acc; bool direct;
+struct SmemTables {
+  using Addr = uint32_t;
+  static __device__ __forceinline__ Addr at(const uint8_t* blob) { return (uint32_t)__cvta_generic_to_shared(blob); }
+  static __device__ __forceinline__ uint32_t u8(Addr a) { return lds_u8(a); }
+  static __device__ __forceinline__ uint32_t u16(Addr a) { return lds_u16(a); }
+  static __device__ __forceinline__ uint32_t u32(Addr a) { return lds_u32(a); }
+};
+struct GlobalTables {
+  using Addr = const uint8_t*;
+  static __device__ __forceinline__ Addr at(const uint8_t* blob) { return blob; }
+  static __device__ __forceinline__ uint32_t u8(Addr a) { return *a; }
+  static __device__ __forceinline__ uint32_t u16(Addr a) { return *reinterpret_cast<const uint16_t*>(a); }
+  static __device__ __forceinline__ uint32_t u32(Addr a) { return *reinterpret_cast<const uint32_t*>(a); }
+};
+
+// One automaton run.  out[] has an entry (0) for every non-accepting state too (feiscan_prog.h), so there is no branch around
+// the lookup and the byte loads of an unrolled group issue ahead of the table walk.
+template <class M> struct Dfa {
+  typename M::Addr trans, out, endout, cls;
+  uint32_t stride2, empty_acc, s, acc;
+  bool direct;
+  __device__ __forceinline__ Dfa(const uint8_t* blob, uint32_t off) {
+    const fei_prog_dfa* d = reinterpret_cast<const fei_prog_dfa*>(blob + off);
+    const typename M::Addr base = M::at(blob);
+    trans = base + d->off_trans; out = base + d->off_out; endout = base + d->off_endout; cls = base + d->off_cls;
+    stride2 = d->row_stride * 2u; empty_acc = d->empty_acc; direct = d->n_cols == 256;
+    s = d->start; acc = M::u32(out + 4u * s);
+  }
   __device__ __forceinline__ void step(uint32_t b) {
-    const uint32_t col = direct ? b : lds_u8(d.cls + b);
-    s = lds_u16(d.trans + s * d.stride2 + col * 2u);
-    acc |= lds_u32(d.out + 4u * s);
+    const uint32_t col = direct ? b : M::u8(cls + b);
+    s = M::u16(trans + s * stride2 + col * 2u);
+    acc |= M::u32(out + 4u * s);
+  }
+  __device__ __forceinline__ uint32_t result() const { return acc | M::u32(endout + 4u * s); }
+  // a byte span.  (Fetching it as aligned 4- or 16-byte words was measured slower on the header workloads: per-lane skip /
+  // tail predicates diverge.)
+  __device__ __forceinline__ uint32_t span(const uint8_t* p, uint32_t len) {
+    if (len == 0) return empty_acc;
+    uint32_t i = 0;
+    for (; i + 4 <= len; i += 4) {
+      const uint32_t b0 = p[i], b1 = p[i + 1], b2 = p[i + 2], b3 = p[i + 3];
+      step(b0); step(b1); step(b2); step(b3);
+    }
+    for (; i < len; ++i) step(p[i]);
+    return result();
+  }
+  // up to 8 bytes held in a register (the flags string of a record: flags8)
+  __device__ __forceinline__ uint32_t u64(unsigned long long bytes, uint32_t len) {
+    if (len == 0) return empty_acc;
+#pragma unroll
+    for (uint32_t k = 0; k < 8; ++k) if (k < len) step((uint32_t)(bytes >> (8 * k)) & 0xFFu);
+    return result();
+  }
+  // a column value: unit k (16 bytes) of the value at base + k * plane_stride (hdir.cu), LDG.128 per unit
+  __device__ __forceinline__ uint32_t units(const uint8_t* base, uint64_t plane_stride, uint32_t len) {
+    if (len == 0) return empty_acc;
+    for (uint32_t k = 0; k * 16 < len; ++k) {
+      const uint4 c = *reinterpret_cast<const uint4*>(base + k * plane_stride);
+      const uint32_t w[4] = {c.x, c.y, c.z, c.w};
+      const uint32_t nb = len - k * 16;
+#pragma unroll
+      for (uint32_t j = 0; j < 16; ++j) if (j < nb) step((w[j >> 2] >> (8 * (j & 3))) & 0xFFu);
+    }
+    return result();
   }
 };
-__device__ __forceinline__ uint32_t dfa_run_s(const DfaViewS& d, const uint8_t* p, uint32_t len) {
-  if (len == 0) return d.empty_acc;
-  DfaStepS r{d, d.start, lds_u32(d.out + 4u * d.start), d.n_cols == 256};
-  uint32_t i = 0;
-  for (; i + 4 <= len; i += 4) {
-    const uint32_t b0 = p[i], b1 = p[i + 1], b2 = p[i + 2], b3 = p[i + 3];
-    r.step(b0); r.step(b1); r.step(b2); r.step(b3);
-  }
-  for (; i < len; ++i) r.step(p[i]);
-  return r.acc | lds_u32(d.endout + 4u * r.s);
+// `run(dfa)` with the tables where they are: `in_smem` is uniform for the grid (stage_prog_head staged the head for every CTA or for none)
+template <class Run> __device__ __forceinline__ uint32_t dfa_run_at(const uint8_t* blob, uint32_t off, bool in_smem, Run run) {
+  if (in_smem) return run(Dfa<SmemTables>(blob, off));
+  return run(Dfa<GlobalTables>(blob, off));
 }
-// the same over up to 8 bytes held in a register (the flags string of a record: flags8)
-__device__ __forceinline__ uint32_t dfa_run_s_u64(const DfaViewS& d, unsigned long long bytes, uint32_t len) {
-  if (len == 0) return d.empty_acc;
-  DfaStepS r{d, d.start, lds_u32(d.out + 4u * d.start), d.n_cols == 256};
-#pragma unroll
-  for (uint32_t k = 0; k < 8; ++k) if (k < len) r.step((uint32_t)(bytes >> (8 * k)) & 0xFFu);
-  return r.acc | lds_u32(d.endout + 4u * r.s);
-}
-// the same over a column value: unit k (16 bytes) of the value at base + k * plane_stride (hdir.cu), LDG.128 per unit
-__device__ __forceinline__ uint32_t dfa_run_units(const DfaViewS& d, const uint8_t* base, uint64_t plane_stride, uint32_t len) {
-  if (len == 0) return d.empty_acc;
-  DfaStepS r{d, d.start, lds_u32(d.out + 4u * d.start), d.n_cols == 256};
-  for (uint32_t k = 0; k * 16 < len; ++k) {
-    const uint4 c = *reinterpret_cast<const uint4*>(base + k * plane_stride);
-    const uint32_t w[4] = {c.x, c.y, c.z, c.w};
-    const uint32_t nb = len - k * 16;
-#pragma unroll
-    for (uint32_t j = 0; j < 16; ++j) if (j < nb) r.step((w[j >> 2] >> (8 * (j & 3))) & 0xFFu);
-  }
-  return r.acc | lds_u32(d.endout + 4u * r.s);
-}
-__device__ uint32_t dfa_run_units_g(const DfaView& d, const uint8_t* base, uint64_t plane_stride, uint32_t len) {   // tables in global memory
-  if (len == 0) return d.empty_acc;
-  uint32_t s = d.start, acc = d.out[s];
-  const bool direct = d.n_cols == 256;
-  for (uint32_t i = 0; i < len; ++i) {
-    const uint32_t b = base[(uint64_t)(i >> 4) * plane_stride + (i & 15)];
-    s = d.trans[s * d.stride + (direct ? b : d.cls[b])];
-    acc |= d.out[s];
-  }
-  return acc | d.endout[s];
-}
-// dispatch: `in_smem` is uniform for the grid (stage_prog_head either staged the head for every CTA or for none)
 __device__ __forceinline__ uint32_t dfa_run_at(const uint8_t* blob, uint32_t off, bool in_smem, const uint8_t* p, uint32_t len) {
-  if (in_smem) return dfa_run_s(dfa_view_s(blob, off), p, len);
-  return dfa_run(dfa_view(blob, off), p, len);
+  return dfa_run_at(blob, off, in_smem, [&](auto d) { return d.span(p, len); });
 }
+
+// ---------------------------------------------------------------- header field lookup
+// A record's header lines, in order, from its directory entries (hdir.cu).  A key is its dictionary slot.
+struct DirLines {
+  using Key = uint32_t;
+  const uint2* ent; uint32_t n_ent; const uint32_t* key_lut;
+  uint32_t j, key, val_off, val_len;
+  __device__ __forceinline__ bool next() {
+    if (j == n_ent) return false;
+    const uint2 e = ent[j++];
+    key = e.x & 0xFFFFu; val_off = e.y; val_len = e.x >> 16;
+    return true;
+  }
+  __device__ __forceinline__ uint32_t key_mask() const { return key_lut[key]; }
+  __device__ __forceinline__ bool same_key(Key k) const { return k == key; }
+  __device__ __forceinline__ bool assigned_later() const {
+    for (uint32_t k = j; k < n_ent; ++k) if ((ent[k].x & 0xFFFFu) == key) return true;
+    return false;
+  }
+};
+// The same lines split from the record's header text (next_header_line), for headers the directory cannot address.  A key is
+// its span (offset, length) in the text; the key automaton gives its slots.
+struct TextLines {
+  using Key = uint2;
+  const uint8_t *h, *p, *end;
+  const uint8_t* prog; uint32_t key_dfa; bool in_smem;
+  Key key; uint32_t val_off, val_len;
+  __device__ __forceinline__ bool next() {
+    for (HeaderLine l; p < end;)
+      if (next_header_line(p, end, l)) {
+        key = make_uint2((uint32_t)(l.ka - h), (uint32_t)(l.kb - l.ka)); val_off = (uint32_t)(l.va - h); val_len = (uint32_t)(l.vb - l.va);
+        return true;
+      }
+    return false;
+  }
+  __device__ __forceinline__ uint32_t key_mask() const { return dfa_run_at(prog, key_dfa, in_smem, h + key.x, key.y); }
+  __device__ __forceinline__ bool same_key(Key k) const {
+    bool same = k.y == key.y;
+    for (uint32_t b = 0; same && b < k.y; ++b) same = h[k.x + b] == h[key.x + b];
+    return same;
+  }
+  __device__ __forceinline__ bool assigned_later() const {
+    HeaderLine l;
+    for (const uint8_t* q = p; q < end;)
+      if (next_header_line(q, end, l) && same_key(make_uint2((uint32_t)(l.ka - h), (uint32_t)(l.kb - l.ka)))) return true;
+    return false;
+  }
+};
+
+// The reference's headers dict (filled line by line by utils.py:113-118, read by search.py:121-132 and utils.py:333-336), asked
+// for program slots 0 .. kSlots-1 over one record's header lines, by the slot's mode(s):
+//   0: the first key whose lower() equals the field fixes the spelling; the value is that of the last line with exactly that spelling;
+//   1: exact key, the last line wins;
+//   2: every value of the dict: each line whose key no later line assigns again goes to any(s, off, len).
+// Returns the mode-0/1 slots found; their values are at val_off[s] / val_len[s] (offsets into the record's header text).  Both
+// line sources give the same answers: k_hdir checks every interned key byte for byte against its slot's spelling.
+template <uint32_t kSlots, class Lines, class Mode, class Any>
+__device__ __forceinline__ uint32_t header_lookup(Lines lines, Mode mode, uint32_t* val_off, uint32_t* val_len, Any any) {
+  typename Lines::Key first_key[kSlots];
+  uint32_t found = 0, have_first = 0;
+  while (lines.next()) {
+    for (uint32_t km = lines.key_mask() & (kSlots < 32 ? (1u << kSlots) - 1u : ~0u); km; km &= km - 1) {
+      const int s = kSlots == 1 ? 0 : __ffs(km) - 1;
+      const uint32_t m = mode(s);
+      if (m == 2) { if (!lines.assigned_later()) any(s, lines.val_off, lines.val_len); continue; }
+      if (m == 0) {
+        if (!(have_first >> s & 1u)) { have_first |= 1u << s; first_key[s] = lines.key; }
+        else if (!lines.same_key(first_key[s])) continue;      // a different spelling of the key: not the dict entry we read
+      }
+      val_off[s] = lines.val_off; val_len[s] = lines.val_len;   // repeated key: last value wins (dict assignment)
+      found |= 1u << s;
+    }
+  }
+  return found;
+}
+__device__ __forceinline__ void no_values(int, uint32_t, uint32_t) {}   // `any` of a lookup without mode-2 slots
 
 // ---------------------------------------------------------------- head kernel
 struct HeadArgs {
@@ -259,8 +309,6 @@ __device__ void head_finish(const HeadArgs& a, uint64_t rec, uint32_t pre, uint3
   uint32_t slot_acc[FEI_MAX_SLOTS];
   uint32_t present = 0;
   if (parse) {
-    uint32_t first_off[FEI_MAX_SLOTS], first_len[FEI_MAX_SLOTS];
-    uint32_t have_first = 0;
     // fields that have a value column: the record's value sits at plane k, offset 16 * rec -- consecutive threads read
     // consecutive units, and neither the directory nor the header text of the record is touched
     bool walk = false;
@@ -272,100 +320,30 @@ __device__ void head_finish(const HeadArgs& a, uint64_t rec, uint32_t pre, uint3
       if (len == kColAbsent) continue;
       if (len == kColWalk) { walk = true; break; }
       const uint8_t* unit = a.col_planes + (uint64_t)col * kColUnits * a.n * 16 + rec * 16;
-      slot_acc[s] = a.prog_in_smem ? dfa_run_units(dfa_view_s(a.prog, slots[s].off_val_dfa), unit, a.n * 16, len)
-                                   : dfa_run_units_g(dfa_view(a.prog, slots[s].off_val_dfa), unit, a.n * 16, len);
+      slot_acc[s] = dfa_run_at(a.prog, slots[s].off_val_dfa, a.prog_in_smem, [&](auto d) { return d.units(unit, a.n * 16, len); });
       present |= 1u << s;
     }
     if (walk) {
-    present = 0;
-    const uint64_t hoff = a.hdr_off[rec];
-    const uint8_t* h = a.hdr + hoff;
-    const uint32_t hlen = (uint32_t)(a.hdr_off[rec + 1] - hoff);
-    const uint2* ent = a.hdir + a.hdir_off[rec];
-    const uint32_t n_ent = (uint32_t)(a.hdir_off[rec + 1] - a.hdir_off[rec]);
-    if (!(n_ent == 1 && ent[0].x == 0xFFFFFFFFu)) {
-      // the usual case: walk the record's header directory (one entry per line with a colon: interned key, stripped value span)
-      uint32_t first_key[FEI_MAX_SLOTS], val_off[FEI_MAX_SLOTS], val_len[FEI_MAX_SLOTS];
+      // the record's header lines: its directory entries, or its text when the directory cannot address it
+      const uint8_t* h = a.hdr + a.hdr_off[rec];
+      const uint2* ent = a.hdir + a.hdir_off[rec];
+      const uint32_t n_ent = (uint32_t)(a.hdir_off[rec + 1] - a.hdir_off[rec]);
+      uint32_t val_off[FEI_MAX_SLOTS], val_len[FEI_MAX_SLOTS];
       uint32_t any_mask = 0;                                   // mode-2 slots ("any header value", utils.py:333-336) already accumulated
-      for (uint32_t j = 0; j < n_ent; ++j) {
-        const uint2 e = ent[j];
-        const uint32_t kid = e.x & 0xFFFFu;
-        uint32_t km = a.key_lut[kid];
-        while (km) {
-          int s = __ffs(km) - 1; km &= km - 1;
-          if (slots[s].mode == 2) {
-            // every value of the headers dict: a line counts unless a later line assigns the same key again
-            bool overridden = false;
-            for (uint32_t k = j + 1; k < n_ent && !overridden; ++k) overridden = (ent[k].x & 0xFFFFu) == kid;
-            if (overridden) continue;
-            const uint32_t acc = dfa_run_at(a.prog, slots[s].off_val_dfa, a.prog_in_smem, h + e.y, e.x >> 16);
-            slot_acc[s] = (any_mask >> s & 1u) ? (slot_acc[s] | acc) : acc;
-            any_mask |= 1u << s;
-            continue;
-          }
-          if (slots[s].mode == 0) {                            // first key that lower()-equals the field (search.py:121-122)
-            if (!(have_first >> s & 1)) { have_first |= 1u << s; first_key[s] = kid; }
-            else if (first_key[s] != kid) continue;            // a different spelling of the key: not the dict entry we read
-          }
-          val_off[s] = e.y; val_len[s] = e.x >> 16;            // repeated key: last value wins (dict assignment)
-          present |= 1u << s;
-        }
-      }
-      for (uint32_t m = present; m;) {
-        int s = __ffs(m) - 1; m &= m - 1;
+      auto any = [&](int s, uint32_t off, uint32_t len) {
+        const uint32_t acc = dfa_run_at(a.prog, slots[s].off_val_dfa, a.prog_in_smem, h + off, len);
+        slot_acc[s] = (any_mask >> s & 1u) ? (slot_acc[s] | acc) : acc;
+        any_mask |= 1u << s;
+      };
+      auto mode = [&](int s) { return slots[s].mode; };
+      present = text_record(ent, n_ent)
+          ? header_lookup<FEI_MAX_SLOTS>(TextLines{h, h, a.hdr + a.hdr_off[rec + 1], a.prog, ph->off_key_dfa, a.prog_in_smem}, mode, val_off, val_len, any)
+          : header_lookup<FEI_MAX_SLOTS>(DirLines{ent, n_ent, a.key_lut}, mode, val_off, val_len, any);
+      for (uint32_t m = present; m; m &= m - 1) {
+        const int s = __ffs(m) - 1;
         slot_acc[s] = dfa_run_at(a.prog, slots[s].off_val_dfa, a.prog_in_smem, h + val_off[s], val_len[s]);
       }
       present |= any_mask;
-    } else {
-    // header text longer than a directory span can address: split / strip it here
-    DfaView keyd = dfa_view(a.prog, ph->off_key_dfa);
-    const uint8_t* hend = h + hlen;
-    const uint8_t* p = h;
-    while (p < hend) {
-      const uint8_t* eol = p; const uint8_t* colon = nullptr;
-      while (eol < hend && *eol != '\n') { if (!colon && *eol == ':') colon = eol; ++eol; }
-      if (colon) {                                             // `if ":" in line` (utils.py:116)
-        const uint8_t* ka = p; const uint8_t* kb = colon; strip_span(ka, kb);
-        const uint8_t* va = colon + 1; const uint8_t* vb = eol; strip_span(va, vb);
-        uint32_t km = dfa_run(keyd, ka, (uint32_t)(kb - ka));
-        while (km) {
-          int s = __ffs(km) - 1; km &= km - 1;
-          if (slots[s].mode == 2) {
-            // every value of the headers dict: this line counts unless a later line assigns the same (stripped) key again
-            bool overridden = false;
-            for (const uint8_t* q = eol + 1; q < hend && !overridden;) {
-              const uint8_t* e2 = q; const uint8_t* c2 = nullptr;
-              while (e2 < hend && *e2 != '\n') { if (!c2 && *e2 == ':') c2 = e2; ++e2; }
-              if (c2) {
-                const uint8_t* k2a = q; const uint8_t* k2b = c2; strip_span(k2a, k2b);
-                bool same = (k2b - k2a) == (kb - ka);
-                for (uint32_t k = 0; same && k < (uint32_t)(kb - ka); ++k) same = k2a[k] == ka[k];
-                overridden = same;
-              }
-              q = e2 + 1;
-            }
-            if (overridden) continue;
-            const uint32_t acc = dfa_run(dfa_view(a.prog, slots[s].off_val_dfa), va, (uint32_t)(vb - va));
-            slot_acc[s] = (present >> s & 1u) ? (slot_acc[s] | acc) : acc;
-            present |= 1u << s;
-            continue;
-          }
-          if (slots[s].mode == 0) {                            // first key that lower()-equals the field (search.py:121-122)
-            if (!(have_first >> s & 1)) { have_first |= 1u << s; first_off[s] = (uint32_t)(ka - h); first_len[s] = (uint32_t)(kb - ka); }
-            else {
-              bool same = first_len[s] == (uint32_t)(kb - ka);
-              for (uint32_t k = 0; same && k < first_len[s]; ++k) same = h[first_off[s] + k] == ka[k];
-              if (!same) continue;                             // a different spelling of the key: not the dict entry we read
-            }
-          }
-          DfaView vd = dfa_view(a.prog, slots[s].off_val_dfa);
-          slot_acc[s] = dfa_run(vd, va, (uint32_t)(vb - va));   // repeated key: last value wins (dict assignment)
-          present |= 1u << s;
-        }
-      }
-      p = eol + 1;
-    }
-    }
     }
   }
   for (uint32_t s = 0; s < nslots; ++s)
@@ -409,7 +387,7 @@ __global__ void k_key_lut(const uint8_t* __restrict__ prog, const uint8_t* __res
   const uint32_t s = blockIdx.x * blockDim.x + threadIdx.x;
   if (s >= kKeySlots) return;
   const fei_prog_hdr* ph = reinterpret_cast<const fei_prog_hdr*>(prog);
-  lut[s] = tag[s] ? dfa_run(dfa_view(prog, ph->off_key_dfa), hdr + rep[s], len[s]) : 0u;
+  lut[s] = tag[s] ? Dfa<GlobalTables>(prog, ph->off_key_dfa).span(hdr + rep[s], len[s]) : 0u;
 }
 
 // One warp, after k_key_lut: a program slot whose field is spelled exactly one way in the whole corpus can be read from that
@@ -471,14 +449,8 @@ __global__ void __launch_bounds__(256, 5) k_head_meta(HeadArgs a, Survivor* __re
   }
   if (ph->off_flags_dfa) {                                     // flags string (search.py:105-106): up to 7 letters in flags8
 #pragma unroll
-    for (int r = 0; r < kMetaPer; ++r) {
-      if (a.prog_in_smem) flags_acc[r] = dfa_run_s_u64(dfa_view_s(a.prog, ph->off_flags_dfa), f8[r], (uint32_t)(f8[r] >> 56));
-      else {
-        uint8_t fb[8];
-        for (int k = 0; k < 7; ++k) fb[k] = (uint8_t)(f8[r] >> (8 * k));
-        flags_acc[r] = dfa_run(dfa_view(a.prog, ph->off_flags_dfa), fb, (uint32_t)(f8[r] >> 56));
-      }
-    }
+    for (int r = 0; r < kMetaPer; ++r)
+      flags_acc[r] = dfa_run_at(a.prog, ph->off_flags_dfa, a.prog_in_smem, [&](auto d) { return d.u64(f8[r], (uint32_t)(f8[r] >> 56)); });
   }
   for (uint32_t q = 0; q < ph->n_queries; ++q) {
     bool ok[kMetaPer];
@@ -1892,12 +1864,10 @@ __global__ void __launch_bounds__(256) k_tok_hist(const uint8_t* __restrict__ hd
   if (i >= n || !(alive[i] & 1u)) return;
   const uint2* ent = hdir + hdir_off[i];
   const uint32_t n_ent = (uint32_t)(hdir_off[i + 1] - hdir_off[i]);
-  if (n_ent == 1 && ent[0].x == 0xFFFFFFFFu) { atomicOr(t.flag, 4u); return; }      // header parsed from its text: not handled here
-  int last = -1;
-  for (uint32_t j = 0; j < n_ent; ++j) if (key_lut[ent[j].x & 0xFFFFu] & 1u) last = (int)j;      // slot 0, repeated key: last value
-  if (last < 0) return;
-  const uint8_t* v = hdr + hdr_off[i] + ent[last].y;
-  const uint32_t vlen = ent[last].x >> 16;
+  if (text_record(ent, n_ent)) { atomicOr(t.flag, 4u); return; }                   // header parsed from its text: not handled here
+  uint32_t voff, vlen;                                                               // slot 0, exact key: the last line wins
+  if (!header_lookup<1>(DirLines{ent, n_ent, key_lut}, [](int) { return 1u; }, &voff, &vlen, no_values)) return;
+  const uint8_t* v = hdr + hdr_off[i] + voff;
   uint32_t pos = 0, idx = 0;
   for (;;) {                                                     // str.split(sep): k separators -> k + 1 pieces, empty ones included
     uint32_t end = pos;
@@ -2019,53 +1989,16 @@ __global__ void __launch_bounds__(256) k_slot_spans(HeadArgs a, uint32_t* __rest
   if (rec >= a.n) return;
   const fei_prog_hdr* ph = reinterpret_cast<const fei_prog_hdr*>(a.prog);
   const fei_prog_slot* slots = reinterpret_cast<const fei_prog_slot*>(a.prog + ph->off_slots);
-  const uint32_t mode = slots[0].mode;
+  const uint32_t m = slots[0].mode == 0 ? 0u : 1u;              // any other mode: exact key, the last line wins
+  auto mode = [m](int) { return m; };
   const uint64_t hoff = a.hdr_off[rec];
   const uint8_t* h = a.hdr + hoff;
-  const uint32_t hlen = (uint32_t)(a.hdr_off[rec + 1] - hoff);
   const uint2* ent = a.hdir + a.hdir_off[rec];
   const uint32_t n_ent = (uint32_t)(a.hdir_off[rec + 1] - a.hdir_off[rec]);
-  bool have = false, have_first = false;
   uint32_t voff = 0, vlen = 0;
-  if (!(n_ent == 1 && ent[0].x == 0xFFFFFFFFu)) {
-    uint32_t first_key = 0;
-    for (uint32_t j = 0; j < n_ent; ++j) {
-      const uint2 e = ent[j];
-      const uint32_t kid = e.x & 0xFFFFu;
-      if (!(a.key_lut[kid] & 1u)) continue;
-      if (mode == 0) {
-        if (!have_first) { have_first = true; first_key = kid; }
-        else if (first_key != kid) continue;
-      }
-      voff = e.y; vlen = e.x >> 16; have = true;
-    }
-  } else {
-    DfaView keyd = dfa_view(a.prog, ph->off_key_dfa);
-    const uint8_t* hend = h + hlen;
-    const uint8_t* p = h;
-    uint32_t first_off = 0, first_len = 0;
-    while (p < hend) {
-      const uint8_t* eol = p; const uint8_t* colon = nullptr;
-      while (eol < hend && *eol != '\n') { if (!colon && *eol == ':') colon = eol; ++eol; }
-      if (colon) {
-        const uint8_t* ka = p; const uint8_t* kb = colon; strip_span(ka, kb);
-        const uint8_t* va = colon + 1; const uint8_t* vb = eol; strip_span(va, vb);
-        if (dfa_run(keyd, ka, (uint32_t)(kb - ka)) & 1u) {
-          bool take = true;
-          if (mode == 0) {
-            if (!have_first) { have_first = true; first_off = (uint32_t)(ka - h); first_len = (uint32_t)(kb - ka); }
-            else {
-              bool same = first_len == (uint32_t)(kb - ka);
-              for (uint32_t k = 0; same && k < first_len; ++k) same = h[first_off + k] == ka[k];
-              take = same;
-            }
-          }
-          if (take) { voff = (uint32_t)(va - h); vlen = (uint32_t)(vb - va); have = true; }
-        }
-      }
-      p = eol + 1;
-    }
-  }
+  const bool have = text_record(ent, n_ent)
+      ? header_lookup<1>(TextLines{h, h, a.hdr + a.hdr_off[rec + 1], a.prog, ph->off_key_dfa, false}, mode, &voff, &vlen, no_values)
+      : header_lookup<1>(DirLines{ent, n_ent, a.key_lut}, mode, &voff, &vlen, no_values);
   len_out[rec] = have ? vlen : 0u;
   src_out[rec] = have ? hoff + voff : ~0ull;                     // ~0: the record has no such header
 }

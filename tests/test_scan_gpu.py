@@ -1,6 +1,9 @@
 """GPU parity of the scan kernels through the C ABI against the oracle (record-level restatement
 of search.py / filter.py) on seeded synthetic corpora plus adversarial records."""
+import contextlib
+import os
 import re
+import struct
 
 import numpy as np
 import pytest
@@ -151,11 +154,45 @@ ADVERSARIAL = [
     ("Tags: Python,\u212aelvin\nPriority: HIGH\n", "kelvin sign tag"),
     ("Subject: caf\u00e9 R\u00c9SUM\u00c9\n", "caf\u00e9 r\u00e9sum\u00e9 \U0001F409 dragon\nline2 react"),
     ("Tags: a\x0bb,\x1cpython\x1f\n", "odd whitespace controls"),
+    ("tags: first\nTAGS: second\ntags: third\nTags: fourth\n", "one key in three spellings: the first one names the dict entry"),
 ]
 
 
-def test_adversarial_records_header_parser_and_unicode(gpu):
+@contextlib.contextmanager
+def _env0(var):
+    os.environ[var] = "0"
+    try:
+        yield
+    finally:
+        del os.environ[var]
+
+
+def _three_loads(recs):
+    """The corpus loaded the three ways its header fields can be read: value columns + directory (default), the in-scan
+    text parser for every record (FEI_HDIR=0; otherwise only > 64 KiB headers take it), the directory walk for every
+    field (FEI_HCOLS=0: no value columns)."""
     from fei_b200.corpus import Corpus
+    loads = {"default": Corpus().load(synth.arrays_from_records(recs))}
+    for var in ("FEI_HDIR", "FEI_HCOLS"):
+        with _env0(var):
+            loads[var] = Corpus().load(synth.arrays_from_records(recs))
+    return loads
+
+
+def _scan_legs(c, prog):
+    """Masks of one program: as built (automata in the shared-memory copy of the program head), with fei_prog_hdr.head_bytes
+    (byte offset 76) set to 0 so that the head kernels read every automaton from global memory, and with the head pass
+    split into the meta kernel + work list + parse kernel (FEI_HEAD_FUSE=0)."""
+    legs = {"smem": c.scan_masks(prog)}
+    in_global = bytearray(prog)
+    struct.pack_into("<I", in_global, 76, 0)
+    legs["global"] = c.scan_masks(bytes(in_global))
+    with _env0("FEI_HEAD_FUSE"):
+        legs["unfused"] = c.scan_masks(prog)
+    return legs
+
+
+def _adversarial_records():
     recs = []
     for i, (h, b) in enumerate(ADVERSARIAL):
         r = synth.record(11, i)
@@ -171,8 +208,12 @@ def test_adversarial_records_header_parser_and_unicode(gpu):
     r = synth.record(11, 99); r["hdr"] = b""; r["body"] = "just text: no separator python".encode(); r["raw_text"] = "just text: no separator python"
     r["bits"] = 1
     recs.append(r)
-    mems = [mo.make_memory(r["filename"], r["folder"], r["status"], r["raw_text"], True) for r in recs]
-    c = Corpus().load(synth.arrays_from_records(recs))
+    return recs, [mo.make_memory(r["filename"], r["folder"], r["status"], r["raw_text"], True) for r in recs]
+
+
+def test_adversarial_records_header_parser_and_unicode(gpu):
+    recs, mems = _adversarial_records()
+    checks = []                                   # (what, program, oracle's record list)
     cases = [
         [("Tags", "has_tag", "python")], [("tags", "has_tag", "final")], [("Tags", "has_tag", "lower")], [("tags", "contains", "c")],
         [("Subject", "=", "beta")], [("subject", "contains", "spaced out")], [("subject", "=", "spaced out")], [("Key", "=", "")],
@@ -185,16 +226,37 @@ def test_adversarial_records_header_parser_and_unicode(gpu):
     ]
     for conds in cases:
         pb = ProgramBuilder(); pb.add_query(_search_prog(conds))
-        got = np.nonzero(c.scan_masks(pb.build()))[0].tolist()
-        want = mo.run_search(mems, [{"field": f, "operator": op, "value": v} for f, op, v in conds])
-        assert got == want, conds
+        checks.append((conds, pb.build(), mo.run_search(mems, [{"field": f, "operator": op, "value": v} for f, op, v in conds])))
     # "any header value" slots (mode 2: the legacy substring search, utils.py:333-336): OR over the values of the headers
     # dict -- a repeated key only counts with its last value -- through the directory walk and the in-scan text parser
     for q in ["python", "a,b", "lower", "final", "big one", "x" * 300, "", "spaced out", "emptykey", "huge"]:
         pb = ProgramBuilder(); pb.add_query([Cond(C_SLOT, pattern=Pattern("contains", q), field="", mode=2)])
-        got = np.nonzero(c.scan_masks(pb.build()))[0].tolist()
-        want = [i for i, m in enumerate(mems) if any(q in v.lower() for v in m["headers"].values())]
-        assert got == want, q
+        checks.append((q, pb.build(), [i for i, m in enumerate(mems) if any(q in v.lower() for v in m["headers"].values())]))
+    for load, c in _three_loads(recs).items():
+        for what, prog, want in checks:
+            for leg, masks in _scan_legs(c, prog).items():
+                assert np.nonzero(masks)[0].tolist() == want, (load, leg, what)
+
+
+def _dict_value(headers, field, mode):
+    """The value of `field` in the headers dict (None: absent): mode 0 the first key whose lower() equals the field
+    (oracle.memdir_oracle.lookup without the date parse), mode 1 headers.get(field)."""
+    if mode == 1:
+        return headers.get(field)
+    return next((v for k, v in headers.items() if k.lower() == field.lower()), None)
+
+
+def test_slot_values_follow_the_headers_dict(gpu):
+    """Corpus.slot_values on every way a header can be read, the > 64 KiB header included: fields repeated in several
+    spellings, missing, empty and longer than a value column."""
+    recs, mems = _adversarial_records()
+    for load, c in _three_loads(recs).items():
+        for field in ["Tags", "tags", "TAGS", "Subject", "subject", "Status", "Key", "Priority", "Filler", "nokey", ""]:
+            for mode in (0, 1):
+                pb = ProgramBuilder(); pb.add_query([Cond(C_SLOT, pattern=Pattern("regex", "", 0), field=field, mode=mode)])
+                present, off, blob = c.slot_values(pb.build())
+                got = [blob[int(off[i]):int(off[i + 1])].tobytes().decode() if present[i] else None for i in range(len(recs))]
+                assert got == [_dict_value(m["headers"], field, mode) for m in mems], (load, field, mode)
 
 
 def test_filter_semantics_negate_and_missing(corpus3k):
@@ -434,11 +496,9 @@ def test_staged_text_and_spans_load_equal_plain_load(gpu):
         bad.load_raw(dict(meta, n=len(recs), raw=scattered, raw_bytes=total - 5000, raw_begin=begin, raw_len=lens))
 
 
-def test_random_headers_differential(gpu):
-    """Seeded fuzz of the device header parser (k_head / k_head_parse) against the oracle: random key spellings,
-    duplicate keys, odd whitespace (incl. multi-byte), missing colons, colons in values, empty keys / values."""
+def _random_header_records():
+    """Random key spellings, duplicate keys, odd whitespace (incl. multi-byte), missing colons, colons in values, empty keys / values."""
     import random
-    from fei_b200.corpus import Corpus
     rng = random.Random(4242)
     keys = ["Tags", "tags", "TAGS", "Subject", "subject", "Status", "status", "Priority", "X-Note", "", " Tags", "Tags ", "Ta gs", "Täg", "Key"]
     ws = ["", " ", "  ", "\t", " ", " ", "\x0b", "\x1c", " \t "]
@@ -464,7 +524,14 @@ def test_random_headers_differential(gpu):
     mems = [mo.make_memory(r["filename"], r["folder"], r["status"], r["raw_text"], True) for r in recs]
     for m, r in zip(mems, recs):
         m["metadata"]["flags"] = list(r["flags"])
-    c = Corpus().load(synth.arrays_from_records(recs))
+    return recs, mems
+
+
+def test_random_headers_differential(gpu):
+    """Seeded fuzz of the device header parser (k_head_meta / k_head_parse) against the oracle."""
+    recs, mems = _random_header_records()
+    loads = _three_loads(recs)
+    c = loads["default"]
     cases = [
         [("Tags", "has_tag", "python")], [("tags", "has_tag", "rust")], [("TAGS", "contains", "b")], [("Tags", "=", "python")], [("Tags", "has_tag", "")],
         [("Status", "=", "done")], [("state", "=", "active")], [("status_value", "contains", "")], [("Subject", "contains", "y:")], [("", "=", "python")],
@@ -481,16 +548,29 @@ def test_random_headers_differential(gpu):
         want = mo.run_search(mems, [{"field": f, "operator": op, "value": v} for f, op, v in conds])
         got = np.nonzero(masks >> np.uint32(q) & np.uint32(1))[0].tolist()
         assert got == want, conds
-    # the same corpus with the header directory switched off (FEI_HDIR=0 at load: every record takes the in-scan text
-    # parser that otherwise only > 64 KiB headers reach): both header paths must give the same masks
-    import os
-    for var in ("FEI_HDIR", "FEI_HCOLS"):      # FEI_HCOLS=0: directory walk for every field (no value columns)
-        os.environ[var] = "0"
-        try:
-            c_alt = Corpus().load(synth.arrays_from_records(recs))
-        finally:
-            del os.environ[var]
-        assert np.array_equal(c_alt.scan_masks(pb.build()), masks), var
+    # every header path (value columns, directory walk, in-scan text parser), automata in shared or global memory, head
+    # pass fused or not: the same masks
+    for load, c_alt in loads.items():
+        for leg, got in _scan_legs(c_alt, pb.build()).items():
+            assert np.array_equal(got, masks), (load, leg)
+
+
+def test_token_histogram_directory_loads_and_text_refusal(gpu):
+    """Corpus.token_histogram of the exact "Tags" header (folders.py:286-292) on the default and FEI_HCOLS=0 loads equals a
+    Python count; with every header parsed from its text (FEI_HDIR=0) it is refused."""
+    recs, mems = _random_header_records()
+    want = {}                                    # token -> [count, first record], in first-occurrence order
+    for i, m in enumerate(mems):
+        if "Tags" in m["headers"]:
+            for tag in [t.strip() for t in m["headers"]["Tags"].split(",")]:
+                want.setdefault(tag.encode(), [0, i])[0] += 1
+    want = [(t, n, first) for t, (n, first) in want.items()]
+    pb = ProgramBuilder(); pb.add_query([Cond(C_SLOT, pattern=Pattern("regex", "", 0), field="Tags", mode=1)])
+    loads = _three_loads(recs)
+    for load in ("default", "FEI_HCOLS"):
+        assert loads[load].token_histogram(pb.build(), ",") == want, load
+    with pytest.raises(NotImplementedError):
+        loads["FEI_HDIR"].token_histogram(pb.build(), ",")
 
 
 def _search_prog2(conds):
