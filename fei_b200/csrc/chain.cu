@@ -340,12 +340,6 @@ static int chain_prepare(fei_chain* ch) {
   return FEI_OK;
 }
 
-static int upload(DevBuf& b, const void* src, size_t bytes, cudaStream_t s) {
-  FEI_TRY(b.ensure(bytes ? bytes : 16));
-  if (bytes) FEI_CUDA(cudaMemcpyAsync(b.p, src, bytes, cudaMemcpyHostToDevice, s));
-  return FEI_OK;
-}
-
 }  // namespace fei
 
 using namespace fei;
@@ -379,12 +373,12 @@ extern "C" int fei_chain_load_msgs(fei_chain* ch, const uint8_t* msgs, const uin
   ch->n = n; ch->first_index = first_index;
   ch->msg_bytes = n ? msg_off[n] - msg_off[0] : 0;
   if (n && msg_off[0] != 0) { set_error("msg_off[0] must be 0"); return FEI_E_BADARG; }
-  FEI_TRY(upload(ch->msgs, msgs, ch->msg_bytes, c.stream));
-  FEI_TRY(upload(ch->msg_off, msg_off, (n + 1) * 8, c.stream));
-  FEI_TRY(upload(ch->hash, hash, n ? hash_off[n] : 0, c.stream));
-  FEI_TRY(upload(ch->hash_off, hash_off, (n + 1) * 8, c.stream));
-  FEI_TRY(upload(ch->prev, prev, n ? prev_off[n] : 0, c.stream));
-  FEI_TRY(upload(ch->prev_off, prev_off, (n + 1) * 8, c.stream));
+  FEI_TRY(upload(ch->msgs, msgs, ch->msg_bytes, 0, c.stream));
+  FEI_TRY(upload(ch->msg_off, msg_off, (n + 1) * 8, 0, c.stream));
+  FEI_TRY(upload(ch->hash, hash, n ? hash_off[n] : 0, 0, c.stream));
+  FEI_TRY(upload(ch->hash_off, hash_off, (n + 1) * 8, 0, c.stream));
+  FEI_TRY(upload(ch->prev, prev, n ? prev_off[n] : 0, 0, c.stream));
+  FEI_TRY(upload(ch->prev_off, prev_off, (n + 1) * 8, 0, c.stream));
   if (n == 0) return FEI_OK;
   return chain_prepare(ch);
 }
@@ -531,14 +525,14 @@ extern "C" int fei_chain_load_cols(fei_chain* ch, const fei_json_col* cols, cons
     const fei_json_col& h = cols[k];
     fei_json_col d; d.tag = nullptr; d.uniform_tag = h.uniform_tag; d.num = nullptr; d.str = nullptr; d.str_off = nullptr;
     if (!h.tag && (h.uniform_tag < FEI_J_NULL || h.uniform_tag > FEI_J_BIGINT)) { set_error("column %d: bad uniform tag %d", k, h.uniform_tag); return FEI_E_BADARG; }
-    if (h.tag) { FEI_TRY(upload(ch->col_tag[k], h.tag, n, s)); d.tag = ch->col_tag[k].as<uint8_t>(); }
-    if (h.num) { FEI_TRY(upload(ch->col_num[k], h.num, n * 8, s)); d.num = ch->col_num[k].as<uint64_t>(); }
+    if (h.tag) { FEI_TRY(upload(ch->col_tag[k], h.tag, n, 0, s)); d.tag = ch->col_tag[k].as<uint8_t>(); }
+    if (h.num) { FEI_TRY(upload(ch->col_num[k], h.num, n * 8, 0, s)); d.num = ch->col_num[k].as<uint64_t>(); }
     if (h.str_off) {
       const uint64_t base = h.str_off[0];
       const uint64_t* off = h.str_off;
       if (base) { rebased[k].resize(n + 1); for (uint64_t i = 0; i <= n; ++i) rebased[k][i] = h.str_off[i] - base; off = rebased[k].data(); }
-      FEI_TRY(upload(ch->col_off[k], off, (n + 1) * 8, s));
-      FEI_TRY(upload(ch->col_str[k], h.str ? h.str + base : nullptr, h.str ? h.str_off[n] - base : 0, s));
+      FEI_TRY(upload(ch->col_off[k], off, (n + 1) * 8, 0, s));
+      FEI_TRY(upload(ch->col_str[k], h.str ? h.str + base : nullptr, h.str ? h.str_off[n] - base : 0, 0, s));
       d.str = ch->col_str[k].as<uint8_t>(); d.str_off = ch->col_off[k].as<uint64_t>();
     }
     dc.c[k] = d;
@@ -559,8 +553,8 @@ extern "C" int fei_chain_load_cols(fei_chain* ch, const fei_json_col* cols, cons
   FEI_TRY(ch->msgs.ensure(total + 16));
   k_json_write<<<g, 128, 0, s>>>(dc, n, ch->msg_off.as<uint64_t>(), ch->msgs.as<uint8_t>());
   FEI_CUDA(cudaGetLastError());
-  FEI_TRY(upload(ch->hash, hash, hash_off[n], s));
-  FEI_TRY(upload(ch->hash_off, hash_off, (n + 1) * 8, s));
+  FEI_TRY(upload(ch->hash, hash, hash_off[n], 0, s));
+  FEI_TRY(upload(ch->hash_off, hash_off, (n + 1) * 8, 0, s));
   // previous_hash strings = column 4, already on the device
   FEI_TRY(ch->prev.ensure(ch->col_str[4].bytes ? ch->col_str[4].bytes : 16));
   FEI_TRY(ch->prev_off.ensure((n + 1) * 8));

@@ -53,6 +53,10 @@ struct DevBuf {
   template <class T> T* as() const { return reinterpret_cast<T*>(p); }
 };
 
+// Queues a host-to-device copy of bytes into b (grown to bytes + zero_slack + 16, so never empty) and zeroes the zero_slack
+// bytes behind them.
+int upload(DevBuf& b, const void* src, size_t bytes, size_t zero_slack, cudaStream_t s);
+
 // process-wide state
 struct Context {
   int device = -1;

@@ -43,6 +43,13 @@ void DevBuf::release() {
 }
 size_t total_device_bytes() { return g_dev_bytes.load(); }
 
+int upload(DevBuf& b, const void* src, size_t bytes, size_t zero_slack, cudaStream_t s) {
+  FEI_TRY(b.ensure(bytes + zero_slack + 16));
+  if (bytes) FEI_CUDA(cudaMemcpyAsync(b.p, src, bytes, cudaMemcpyHostToDevice, s));
+  if (zero_slack) FEI_CUDA(cudaMemsetAsync((uint8_t*)b.p + bytes, 0, zero_slack, s));
+  return FEI_OK;
+}
+
 /* The CUDA "current device" is per host thread: a worker thread of the caller (a thread pool loading batches, Flask's request
  * threads) starts on device 0 whatever fei_init bound.  Every path that touches the device goes through ctx() or DevBuf::alloc, so
  * this is where the calling thread is put on the bound device. */

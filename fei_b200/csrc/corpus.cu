@@ -58,18 +58,6 @@ k_window_sort(const uint32_t* __restrict__ len, uint64_t n, uint32_t* __restrict
   }
 }
 
-__device__ __forceinline__ uint4 load16_unaligned(const uint8_t* s) {
-  // assemble 16 bytes from 4-byte aligned loads (the blob has >= 32 bytes of slack at the end)
-  uintptr_t a = reinterpret_cast<uintptr_t>(s);
-  const uint32_t* w = reinterpret_cast<const uint32_t*>(a & ~uintptr_t(3));
-  uint32_t sh = (uint32_t)(a & 3) * 8;
-  uint32_t w0 = w[0], w1 = w[1], w2 = w[2], w3 = w[3], w4 = sh ? w[4] : 0;
-  uint4 r;
-  r.x = __funnelshift_r(w0, w1, sh); r.y = __funnelshift_r(w1, w2, sh);
-  r.z = __funnelshift_r(w2, w3, sh); r.w = __funnelshift_r(w3, w4, sh);
-  return r;
-}
-
 __device__ __forceinline__ uint32_t mask_bytes(uint32_t w, int keep) {   // keep the low `keep` bytes (0..4)
   return keep >= 4 ? w : keep <= 0 ? 0u : (w & ((1u << (8 * keep)) - 1u));
 }
@@ -90,7 +78,7 @@ __global__ void k_tile_copy(const uint8_t* __restrict__ body, const uint64_t* __
   for (uint32_t k = 0; k < maxu; ++k) {
     uint32_t m = __popc(__ballot_sync(0xffffffffu, k < units));
     if (k < units) {
-      uint4 v = load16_unaligned(src + (uint64_t)k * 16);
+      uint4 v = load16(src + (uint64_t)k * 16);
       int rem = (int)len - (int)(k * 16);
       if (rem < 16) { v.x = mask_bytes(v.x, rem); v.y = mask_bytes(v.y, rem - 4); v.z = mask_bytes(v.z, rem - 8); v.w = mask_bytes(v.w, rem - 12); }
       v.x = tile_byte_perm4(v.x); v.y = tile_byte_perm4(v.y); v.z = tile_byte_perm4(v.z); v.w = tile_byte_perm4(v.w);
@@ -100,25 +88,77 @@ __global__ void k_tile_copy(const uint8_t* __restrict__ body, const uint64_t* __
   }
 }
 
-// Inverse (fetch / debugging): thread per record copies its units back to a canonical blob.
-__global__ void k_untile(const uint8_t* __restrict__ tiles, const uint64_t* __restrict__ grp_base,
-                         const uint32_t* __restrict__ grp_len, const uint32_t* __restrict__ rec_pos,
-                         uint64_t first, uint64_t n, const uint64_t* __restrict__ out_off, uint8_t* __restrict__ out) {
-  uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  uint32_t pos = rec_pos[first + i];
-  uint64_t g = pos >> 5; int lane = pos & 31;
-  uint32_t len = grp_len[pos];
+// ---------------------------------------------------------------- fetch: record i of a fetch is idx[i], or first + i when idx is null
+__global__ void k_rec_lens(const uint64_t* __restrict__ idx, uint64_t first, uint64_t m, const uint64_t* __restrict__ hdr_off,
+                           const uint32_t* __restrict__ rec_pos, const uint32_t* __restrict__ grp_len, uint32_t* __restrict__ hlen,
+                           uint32_t* __restrict__ blen) {
+  const uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
+  if (i >= m) return;
+  const uint64_t r = idx ? idx[i] : first + i;
+  hlen[i] = (uint32_t)(hdr_off[r + 1] - hdr_off[r]);
+  blen[i] = grp_len[rec_pos[r]];
+}
+__global__ void k_copy_hdr(const uint64_t* __restrict__ idx, uint64_t m, const uint8_t* __restrict__ hdr, const uint64_t* __restrict__ hdr_off,
+                           const uint64_t* __restrict__ out_off, uint8_t* __restrict__ out) {
+  const uint64_t i = (blockIdx.x * (uint64_t)blockDim.x + threadIdx.x) >> 5;       // a warp per record
+  const int lane = threadIdx.x & 31;
+  if (i >= m) return;
+  const uint64_t r = idx[i];
+  const uint8_t* p = hdr + hdr_off[r];
+  const uint32_t len = (uint32_t)(hdr_off[r + 1] - hdr_off[r]);
+  uint8_t* d = out + out_off[i];
+  for (uint32_t k = lane; k < len; k += 32) d[k] = p[k];
+}
+// Inverse of the tiler: a thread per record copies its units back to a canonical blob.
+__global__ void k_untile_idx(const uint8_t* __restrict__ tiles, const uint64_t* __restrict__ grp_base, const uint32_t* __restrict__ grp_len,
+                             const uint32_t* __restrict__ rec_pos, const uint64_t* __restrict__ idx, uint64_t first, uint64_t m,
+                             const uint64_t* __restrict__ out_off, uint8_t* __restrict__ out) {
+  const uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
+  if (i >= m) return;
+  const uint32_t pos = rec_pos[idx ? idx[i] : first + i];
+  const uint64_t g = pos >> 5; const int lane = pos & 31;
+  const uint32_t len = grp_len[pos];
   const uint32_t* gl = grp_len + g * 32;
   uint8_t* dst = out + out_off[i];
   const uint8_t* gb = tiles + grp_base[g] * 16;
+  uint32_t units[32];
+  for (int l = 0; l < 32; ++l) units[l] = (gl[l] + 15) >> 4;
   for (uint32_t k = 0; k * 16 < len; ++k) {
     uint64_t before = 0;                                      // sum over lanes of min(units, k)
-    for (int l = 0; l < 32; ++l) { uint32_t u = (gl[l] + 15) >> 4; before += u < k ? u : k; }
+    for (int l = 0; l < 32; ++l) before += units[l] < k ? units[l] : k;
     const uint8_t* p = gb + before * 16 + lane * 16;
-    uint32_t cnt = len - k * 16 < 16 ? len - k * 16 : 16;
-    for (uint32_t b = 0; b < cnt; ++b) { uint8_t t = p[b]; dst[k * 16 + b] = (uint8_t)(t ^ ((t >> 1) & 0x20)); }   // undo the tile byte permutation
+    const uint32_t cnt = len - k * 16 < 16 ? len - k * 16 : 16;
+    for (uint32_t b = 0; b < cnt; ++b) dst[k * 16 + b] = tile_byte_unperm(p[b]);
   }
+}
+
+// Offsets [m + 1] of the fetched records' headers and bodies, computed on the device: into d_hoff / d_boff for the copy
+// kernels and into hdr_off / body_off on the host.  Synchronises s.
+static int fetch_offsets(fei_corpus* c, const uint64_t* d_idx, uint64_t first, uint64_t m, DevBuf& d_hoff, DevBuf& d_boff,
+                         uint64_t* hdr_off, uint64_t* body_off, cudaStream_t s) {
+  DevBuf d_hlen, d_blen;
+  FEI_TRY(d_hlen.alloc(m * 4)); FEI_TRY(d_blen.alloc(m * 4)); FEI_TRY(d_hoff.alloc((m + 1) * 8)); FEI_TRY(d_boff.alloc((m + 1) * 8));
+  k_rec_lens<<<(unsigned)((m + 127) / 128), 128, 0, s>>>(d_idx, first, m, c->hdr_off.as<uint64_t>(), c->rec_pos.as<uint32_t>(), c->grp_len.as<uint32_t>(),
+                                                         d_hlen.as<uint32_t>(), d_blen.as<uint32_t>());
+  FEI_TRY(exclusive_scan_u32_u64(d_hlen.as<uint32_t>(), m, d_hoff.as<uint64_t>(), c->scan_tmp, s));
+  FEI_TRY(exclusive_scan_u32_u64(d_blen.as<uint32_t>(), m, d_boff.as<uint64_t>(), c->scan_tmp, s));
+  FEI_CUDA(cudaMemcpyAsync(hdr_off, d_hoff.p, (m + 1) * 8, cudaMemcpyDeviceToHost, s));
+  FEI_CUDA(cudaMemcpyAsync(body_off, d_boff.p, (m + 1) * 8, cudaMemcpyDeviceToHost, s));
+  FEI_CUDA(cudaStreamSynchronize(s));
+  return FEI_OK;
+}
+
+// The bodies of the fetched records, un-tiled on the device into body[0, bytes).  Synchronises s.
+static int fetch_bodies(fei_corpus* c, const uint64_t* d_idx, uint64_t first, uint64_t m, const DevBuf& d_boff, uint8_t* body, uint64_t bytes,
+                        cudaStream_t s) {
+  DevBuf d_b;
+  FEI_TRY(d_b.alloc(bytes + 16));
+  k_untile_idx<<<(unsigned)((m + 127) / 128), 128, 0, s>>>(c->tiles.as<uint8_t>(), c->grp_base.as<uint64_t>(), c->grp_len.as<uint32_t>(), c->rec_pos.as<uint32_t>(),
+                                                           d_idx, first, m, d_boff.as<uint64_t>(), d_b.as<uint8_t>());
+  FEI_CUDA(cudaGetLastError());
+  FEI_CUDA(cudaMemcpyAsync(body, d_b.p, bytes, cudaMemcpyDeviceToHost, s));
+  FEI_CUDA(cudaStreamSynchronize(s));
+  return FEI_OK;
 }
 
 int corpus_load_events(fei_corpus* c) {
@@ -130,7 +170,7 @@ cudaStream_t corpus_load_stream(fei_corpus* c) {
   return c->load_stream ? c->load_stream : ctx().copy_stream;
 }
 
-int build_tiles(fei_corpus* c, const uint8_t* d_body, const uint64_t* d_body_off, cudaStream_t s) {
+static int build_tiles(fei_corpus* c, const uint8_t* d_body, const uint64_t* d_body_off, cudaStream_t s) {
   uint64_t n = c->n;
   uint64_t n_windows = (n + kWindow - 1) / kWindow;
   uint64_t n_groups = n_windows * (kWindow / 32);
@@ -185,10 +225,38 @@ __global__ void k_synth_write(uint64_t seed, uint64_t first, uint64_t n, const u
   fsb[i] = (uint32_t)m.folder | ((uint32_t)m.status << 16);
 }
 
-static int upload(DevBuf& b, const void* src, size_t bytes, size_t slack, cudaStream_t s) {
-  FEI_TRY(b.ensure(bytes + slack + 16));
-  if (bytes) FEI_CUDA(cudaMemcpyAsync(b.p, src, bytes, cudaMemcpyHostToDevice, s));
-  if (slack) FEI_CUDA(cudaMemsetAsync((uint8_t*)b.p + bytes, 0, slack, s));
+int check_load(uint64_t n, const fei_corpus_host* h) {
+  FEI_TRY(require_ready());
+  if (n >= 0xFFFFFFFFull) { set_error("at most 2^32-2 records per shard"); return FEI_E_BADARG; }
+  if (h && n && (!h->ts || !h->wall || !h->flags8 || !h->fsb)) { set_error("missing meta array"); return FEI_E_BADARG; }
+  return FEI_OK;
+}
+
+int upload_meta(fei_corpus* c, const fei_corpus_host* h, cudaStream_t s) {
+  const uint64_t n = h->n;
+  FEI_TRY(upload(c->ts, h->ts, n * 8, 0, s)); FEI_TRY(upload(c->wall, h->wall, n * 8, 0, s));
+  FEI_TRY(upload(c->flags8, h->flags8, n * 8, 0, s)); FEI_TRY(upload(c->fsb, h->fsb, n * 4, 0, s));
+  if (h->name && h->name_off && h->name_spans && n) {
+    c->name_bytes = h->name_off[n];
+    FEI_TRY(upload(c->name, h->name, c->name_bytes, kBlobSlack, s));
+    FEI_TRY(upload(c->name_off, h->name_off, (n + 1) * 8, 0, s));
+    FEI_TRY(upload(c->name_spans, h->name_spans, n * 8, 0, s));
+  } else { c->name.release(); c->name_off.release(); c->name_spans.release(); c->name_bytes = 0; }
+  return FEI_OK;
+}
+
+// Once the tiles hold the text, the canonical staging text (body, its offsets and the raw file text of fei_corpus_load_raw) is
+// kept for the next load while it is small, so that streamed batches reuse it without a cudaMalloc / cudaFree (a cudaFree
+// synchronises the device), and dropped when the caller asks or when it passes 8 GiB, so that HBM holds one copy of a big
+// resident corpus' text.  It goes before the header directory, which reads only hdr.
+int pack_canonical(fei_corpus* c, DevBuf& body, DevBuf& body_off, cudaStream_t s, bool drop_text, cudaEvent_t packed) {
+  FEI_TRY(build_tiles(c, body.as<uint8_t>(), body_off.as<uint64_t>(), s));
+  drop_text = drop_text || body.bytes > (8ull << 30);
+  if (drop_text) { body.release(); body_off.release(); c->stage_raw.release(); c->staged_text_bytes = ~0ull; }
+  FEI_TRY(build_header_dir(c, s));
+  if (packed) FEI_CUDA(cudaEventRecord(packed, s));
+  if (drop_text) { c->tmp_len.release(); c->tmp_gunits.release(); }
+  c->loaded = true;
   return FEI_OK;
 }
 
@@ -217,13 +285,10 @@ extern "C" int fei_corpus_destroy(fei_corpus* c) {
 }
 
 extern "C" int fei_corpus_load(fei_corpus* c, const fei_corpus_host* h) {
-  if (!c) { set_error("null corpus"); return FEI_E_BADARG; }
-  std::lock_guard<std::mutex> lock(c->mu);
-  FEI_TRY(require_ready());
   if (!c || !h) { set_error("null argument"); return FEI_E_BADARG; }
-  if (h->n >= 0xFFFFFFFFull) { set_error("at most 2^32-2 records per shard"); return FEI_E_BADARG; }
-  if (h->n && (!h->hdr_off || !h->body_off || !h->ts || !h->wall || !h->flags8 || !h->fsb)) { set_error("missing corpus array"); return FEI_E_BADARG; }
-  Context& cx = ctx();
+  std::lock_guard<std::mutex> lock(c->mu);
+  FEI_TRY(check_load(h->n, h));
+  if (h->n && (!h->hdr_off || !h->body_off)) { set_error("missing corpus array"); return FEI_E_BADARG; }
   cudaStream_t s = corpus_load_stream(c);            // see fei_corpus_load_raw: loads overlap scans (and loads) of other handles
   uint64_t n = h->n;
   c->n = n; c->global_base = h->global_base; c->loaded = false;
@@ -231,44 +296,26 @@ extern "C" int fei_corpus_load(fei_corpus* c, const fei_corpus_host* h) {
   const uint64_t* hoff = n ? h->hdr_off : zero_off;
   const uint64_t* boff = n ? h->body_off : zero_off;
   if (hoff[0] != 0 || boff[0] != 0) { set_error("offset arrays must start at 0"); return FEI_E_BADARG; }
-  c->hdr_bytes = hoff[n]; c->body_bytes = boff[n];
-  FEI_CUDA(cudaEventRecord(c->ev[0], s));
-  FEI_TRY(upload(c->hdr, h->hdr, c->hdr_bytes, 32, s));
-  FEI_TRY(upload(c->hdr_off, hoff, (n + 1) * 8, 0, s));
-  FEI_TRY(upload(c->ts, h->ts, n * 8, 0, s));
-  FEI_TRY(upload(c->wall, h->wall, n * 8, 0, s));
-  FEI_TRY(upload(c->flags8, h->flags8, n * 8, 0, s));
-  FEI_TRY(upload(c->fsb, h->fsb, n * 4, 0, s));
-  if (h->name && h->name_off && h->name_spans && n) {
-    c->name_bytes = h->name_off[n];
-    FEI_TRY(upload(c->name, h->name, c->name_bytes, 32, s));
-    FEI_TRY(upload(c->name_off, h->name_off, (n + 1) * 8, 0, s));
-    FEI_TRY(upload(c->name_spans, h->name_spans, n * 8, 0, s));
-  } else { c->name.release(); c->name_off.release(); c->name_spans.release(); c->name_bytes = 0; }
   for (uint64_t i = 0; i < n; ++i)
     if (boff[i + 1] - boff[i] > (32u << 20)) { set_error("record %llu: body larger than 32 MiB is not supported", (unsigned long long)i); return FEI_E_UNSUPPORTED; }
-  DevBuf& body = c->stage_body; DevBuf& body_off = c->stage_body_off;
-  FEI_TRY(upload(body, h->body, c->body_bytes, 32, s));
-  FEI_TRY(upload(body_off, boff, (n + 1) * 8, 0, s));
+  c->hdr_bytes = hoff[n]; c->body_bytes = boff[n];
+  FEI_CUDA(cudaEventRecord(c->ev[0], s));
+  FEI_TRY(upload_meta(c, h, s));                     // the small arrays before the text, like fei_corpus_load_raw
+  FEI_TRY(upload(c->hdr, h->hdr, c->hdr_bytes, kBlobSlack, s));
+  FEI_TRY(upload(c->hdr_off, hoff, (n + 1) * 8, 0, s));
+  FEI_TRY(upload(c->stage_body, h->body, c->body_bytes, kBlobSlack, s));
+  FEI_TRY(upload(c->stage_body_off, boff, (n + 1) * 8, 0, s));
   FEI_CUDA(cudaEventRecord(c->ev[1], s));
-  FEI_TRY(build_tiles(c, body.as<uint8_t>(), body_off.as<uint64_t>(), s));
-  FEI_TRY(build_header_dir(c, s));
-  // the canonical body is only a staging area: keep it for the next batch when it is small (streaming
-  // loads of host batches), drop it for big resident corpora so HBM holds one copy of the text
-  if (body.bytes > (8ull << 30)) { body.release(); body_off.release(); c->tmp_len.release(); c->tmp_gunits.release(); }
+  FEI_TRY(pack_canonical(c, c->stage_body, c->stage_body_off, s, false, nullptr));
   FEI_CUDA(cudaEventElapsedTime(&c->timing.h2d_ms, c->ev[0], c->ev[1]));
-  c->loaded = true;
   return FEI_OK;
 }
 
 extern "C" int fei_corpus_synth(fei_corpus* c, uint64_t seed, uint64_t first, uint64_t n) {
   if (!c) { set_error("null corpus"); return FEI_E_BADARG; }
   std::lock_guard<std::mutex> lock(c->mu);
-  FEI_TRY(require_ready());
-  if (!c) { set_error("null corpus"); return FEI_E_BADARG; }
-  if (n >= 0xFFFFFFFFull) { set_error("at most 2^32-2 records per shard"); return FEI_E_BADARG; }
-  Context& cx = ctx();
-  cudaStream_t s = cx.stream;
+  FEI_TRY(check_load(n, nullptr));
+  cudaStream_t s = ctx().stream;
   c->n = n; c->global_base = first; c->loaded = false;
   c->name.release(); c->name_off.release(); c->name_spans.release(); c->name_bytes = 0;
   DevBuf hlen, blen, body, body_off;
@@ -284,18 +331,15 @@ extern "C" int fei_corpus_synth(fei_corpus* c, uint64_t seed, uint64_t first, ui
   FEI_CUDA(cudaMemcpyAsync(&hb, c->hdr_off.as<uint64_t>() + n, 8, cudaMemcpyDeviceToHost, s));
   FEI_CUDA(cudaMemcpyAsync(&bb, body_off.as<uint64_t>() + n, 8, cudaMemcpyDeviceToHost, s));
   FEI_CUDA(cudaStreamSynchronize(s));
+  hlen.release(); blen.release();
   c->hdr_bytes = hb; c->body_bytes = bb;
-  FEI_TRY(c->hdr.alloc(hb + 48)); FEI_TRY(body.alloc(bb + 48));
-  FEI_CUDA(cudaMemsetAsync((uint8_t*)c->hdr.p + hb, 0, 48, s));
-  FEI_CUDA(cudaMemsetAsync((uint8_t*)body.p + bb, 0, 48, s));
+  FEI_TRY(c->hdr.alloc(hb + kBlobSlack)); FEI_TRY(body.alloc(bb + kBlobSlack));
+  FEI_CUDA(cudaMemsetAsync((uint8_t*)c->hdr.p + hb, 0, kBlobSlack, s));
+  FEI_CUDA(cudaMemsetAsync((uint8_t*)body.p + bb, 0, kBlobSlack, s));
   if (n) k_synth_write<<<g, 128, 0, s>>>(seed, first, n, c->hdr_off.as<uint64_t>(), body_off.as<uint64_t>(), c->hdr.as<uint8_t>(), body.as<uint8_t>(),
                                          c->ts.as<int64_t>(), c->wall.as<int64_t>(), c->flags8.as<uint64_t>(), c->fsb.as<uint32_t>());
   FEI_CUDA(cudaGetLastError());
-  FEI_TRY(build_tiles(c, body.as<uint8_t>(), body_off.as<uint64_t>(), s));
-  body.release(); body_off.release(); hlen.release(); blen.release();   // the tiles hold the text now; free it before the header directory
-  FEI_TRY(build_header_dir(c, s));
-  c->loaded = true;
-  return FEI_OK;
+  return pack_canonical(c, body, body_off, s, true, nullptr);
 }
 
 extern "C" int fei_corpus_stats_get(const fei_corpus* c, fei_corpus_stats* out) {
@@ -316,43 +360,61 @@ extern "C" int fei_corpus_fetch(fei_corpus* c, uint64_t first, uint64_t n,
   if (!c) { set_error("null corpus"); return FEI_E_BADARG; }
   std::lock_guard<std::mutex> lock(c->mu);
   FEI_TRY(require_ready());
-  if (!c || !c->loaded) { set_error("corpus not loaded"); return FEI_E_STATE; }
+  if (!c->loaded) { set_error("corpus not loaded"); return FEI_E_STATE; }
   if (first + n > c->n) { set_error("range out of bounds"); return FEI_E_BADARG; }
   if (n == 0) return FEI_OK;
   cudaStream_t s = ctx().stream;
-  std::vector<uint64_t> ho(n + 1);
-  FEI_CUDA(cudaMemcpyAsync(ho.data(), c->hdr_off.as<uint64_t>() + first, (n + 1) * 8, cudaMemcpyDeviceToHost, s));
-  FEI_CUDA(cudaStreamSynchronize(s));
-  if (hdr_off) for (uint64_t i = 0; i <= n; ++i) hdr_off[i] = ho[i] - ho[0];
+  uint64_t h0 = 0;
+  std::vector<uint64_t> ho, bo;
+  DevBuf d_hoff, d_boff;
+  if (hdr || hdr_off || body || body_off) {          // not for the meta columns alone
+    ho.resize(n + 1); bo.resize(n + 1);
+    FEI_CUDA(cudaMemcpyAsync(&h0, c->hdr_off.as<uint64_t>() + first, 8, cudaMemcpyDeviceToHost, s));
+    FEI_TRY(fetch_offsets(c, nullptr, first, n, d_hoff, d_boff, ho.data(), bo.data(), s));
+  }
+  if (hdr_off) memcpy(hdr_off, ho.data(), (n + 1) * 8);
   if (hdr) {
-    if (ho[n] - ho[0] > hdr_cap) { set_error("header buffer too small: need %llu", (unsigned long long)(ho[n] - ho[0])); return FEI_E_CAPACITY; }
-    FEI_CUDA(cudaMemcpyAsync(hdr, c->hdr.as<uint8_t>() + ho[0], ho[n] - ho[0], cudaMemcpyDeviceToHost, s));
+    if (ho[n] > hdr_cap) { set_error("header buffer too small: need %llu", (unsigned long long)ho[n]); return FEI_E_CAPACITY; }
+    FEI_CUDA(cudaMemcpyAsync(hdr, c->hdr.as<uint8_t>() + h0, ho[n], cudaMemcpyDeviceToHost, s));
   }
   if (ts) FEI_CUDA(cudaMemcpyAsync(ts, c->ts.as<int64_t>() + first, n * 8, cudaMemcpyDeviceToHost, s));
   if (wall) FEI_CUDA(cudaMemcpyAsync(wall, c->wall.as<int64_t>() + first, n * 8, cudaMemcpyDeviceToHost, s));
   if (flags8) FEI_CUDA(cudaMemcpyAsync(flags8, c->flags8.as<uint64_t>() + first, n * 8, cudaMemcpyDeviceToHost, s));
   if (fsb) FEI_CUDA(cudaMemcpyAsync(fsb, c->fsb.as<uint32_t>() + first, n * 4, cudaMemcpyDeviceToHost, s));
-  if (body || body_off) {
-    // lengths via rec_pos -> grp_len
-    std::vector<uint32_t> pos(n), glen(c->n_groups * 32);
-    FEI_CUDA(cudaMemcpyAsync(pos.data(), c->rec_pos.as<uint32_t>() + first, n * 4, cudaMemcpyDeviceToHost, s));
-    FEI_CUDA(cudaMemcpyAsync(glen.data(), c->grp_len.p, glen.size() * 4, cudaMemcpyDeviceToHost, s));
-    FEI_CUDA(cudaStreamSynchronize(s));
-    std::vector<uint64_t> bo(n + 1, 0);
-    for (uint64_t i = 0; i < n; ++i) bo[i + 1] = bo[i] + glen[pos[i]];
-    if (body_off) memcpy(body_off, bo.data(), (n + 1) * 8);
-    if (body) {
-      if (bo[n] > body_cap) { set_error("body buffer too small: need %llu", (unsigned long long)bo[n]); return FEI_E_CAPACITY; }
-      DevBuf d_off, d_out;
-      FEI_TRY(d_off.alloc((n + 1) * 8)); FEI_TRY(d_out.alloc(bo[n] + 16));
-      FEI_CUDA(cudaMemcpyAsync(d_off.p, bo.data(), (n + 1) * 8, cudaMemcpyHostToDevice, s));
-      k_untile<<<(unsigned)((n + 127) / 128), 128, 0, s>>>(c->tiles.as<uint8_t>(), c->grp_base.as<uint64_t>(), c->grp_len.as<uint32_t>(),
-                                                        c->rec_pos.as<uint32_t>(), first, n, d_off.as<uint64_t>(), d_out.as<uint8_t>());
-      FEI_CUDA(cudaGetLastError());
-      FEI_CUDA(cudaMemcpyAsync(body, d_out.p, bo[n], cudaMemcpyDeviceToHost, s));
-      FEI_CUDA(cudaStreamSynchronize(s));
-    }
+  if (body_off) memcpy(body_off, bo.data(), (n + 1) * 8);
+  if (body) {
+    if (bo[n] > body_cap) { set_error("body buffer too small: need %llu", (unsigned long long)bo[n]); return FEI_E_CAPACITY; }
+    FEI_TRY(fetch_bodies(c, nullptr, first, n, d_boff, body, bo[n], s));
   }
   FEI_CUDA(cudaStreamSynchronize(s));
+  return FEI_OK;
+}
+
+/* Header text and body of the m records idx[0..m) (any order, repeats allowed), for materialising hits: hdr_off / body_off get
+ * m + 1 offsets; FEI_E_CAPACITY (needed sizes in hdr_off[m] / body_off[m]) when a blob is too small.  hdr / body may be NULL to
+ * only size the buffers.                                                                                                         */
+extern "C" int fei_corpus_fetch_records(fei_corpus* c, const uint64_t* idx, uint64_t m, uint8_t* hdr, uint64_t hdr_cap, uint64_t* hdr_off,
+                                        uint8_t* body, uint64_t body_cap, uint64_t* body_off) {
+  if (!c || (m && !idx) || !hdr_off || !body_off) { set_error("null argument"); return FEI_E_BADARG; }
+  std::lock_guard<std::mutex> lock(c->mu);
+  FEI_TRY(require_ready());
+  if (!c->loaded) { set_error("corpus not loaded"); return FEI_E_STATE; }
+  hdr_off[0] = 0; body_off[0] = 0;
+  if (m == 0) return FEI_OK;
+  for (uint64_t i = 0; i < m; ++i) if (idx[i] >= c->n) { set_error("record index %llu out of range", (unsigned long long)idx[i]); return FEI_E_BADARG; }
+  cudaStream_t s = ctx().stream;
+  DevBuf d_idx, d_hoff, d_boff, d_h;
+  FEI_TRY(d_idx.alloc(m * 8));
+  FEI_CUDA(cudaMemcpyAsync(d_idx.p, idx, m * 8, cudaMemcpyHostToDevice, s));
+  FEI_TRY(fetch_offsets(c, d_idx.as<uint64_t>(), 0, m, d_hoff, d_boff, hdr_off, body_off, s));
+  if ((hdr && hdr_off[m] > hdr_cap) || (body && body_off[m] > body_cap)) { set_error("fetch buffers too small: need %llu header and %llu body bytes", (unsigned long long)hdr_off[m], (unsigned long long)body_off[m]); return FEI_E_CAPACITY; }
+  if (hdr && hdr_off[m]) {
+    FEI_TRY(d_h.alloc(hdr_off[m] + 16));
+    k_copy_hdr<<<(unsigned)((m * 32 + 255) / 256), 256, 0, s>>>(d_idx.as<uint64_t>(), m, c->hdr.as<uint8_t>(), c->hdr_off.as<uint64_t>(), d_hoff.as<uint64_t>(), d_h.as<uint8_t>());
+    FEI_CUDA(cudaMemcpyAsync(hdr, d_h.p, hdr_off[m], cudaMemcpyDeviceToHost, s));
+  }
+  if (body && body_off[m]) FEI_TRY(fetch_bodies(c, d_idx.as<uint64_t>(), 0, m, d_boff, body, body_off[m], s));
+  FEI_CUDA(cudaStreamSynchronize(s));
+  FEI_CUDA(cudaGetLastError());
   return FEI_OK;
 }

@@ -27,6 +27,21 @@ namespace fei {
 // space / punctuation banks 16-31 (measured: 2.0 -> see DESIGN.md wavefronts per lookup on single-pattern scans).
 #ifdef __CUDACC__
 __host__ __device__ __forceinline__ uint32_t tile_byte_perm4(uint32_t w) { return w ^ ((w >> 1) & 0x20202020u); }
+// the inverse of one stored byte (the permutation is its own inverse)
+__host__ __device__ __forceinline__ uint8_t tile_byte_unperm(uint8_t t) { return (uint8_t)tile_byte_perm4(t); }
+#endif
+// Zero-filled bytes behind the header blob and the canonical staging body of every load.  load16(p) reads the 20 bytes from
+// p rounded down to 4, and the tiler and the value columns call it at any p inside a value: up to 19 bytes past the blob.
+constexpr uint64_t kBlobSlack = 32;
+#ifdef __CUDACC__
+// 16 bytes from any address, assembled from 4-byte aligned loads
+__device__ __forceinline__ uint4 load16(const uint8_t* s) {
+  const uintptr_t a = reinterpret_cast<uintptr_t>(s);
+  const uint32_t* w = reinterpret_cast<const uint32_t*>(a & ~uintptr_t(3));
+  const uint32_t sh = (uint32_t)(a & 3) * 8;
+  const uint32_t w0 = w[0], w1 = w[1], w2 = w[2], w3 = w[3], w4 = sh ? w[4] : 0;
+  return make_uint4(__funnelshift_r(w0, w1, sh), __funnelshift_r(w1, w2, sh), __funnelshift_r(w2, w3, sh), __funnelshift_r(w3, w4, sh));
+}
 #endif
 constexpr int kWindow = 4096;
 constexpr uint32_t kKeySlots = 4096;       // header-key dictionary slots (hdir.cu); at most half may fill
@@ -65,7 +80,7 @@ struct fei_corpus {
   bool has_text_records = false;         // some record's header is parsed from its text (keys not in the dictionary)
   fei::DevBuf stage_body, stage_body_off, tmp_len, tmp_gunits;   // reused by repeated loads (no cudaMalloc per batch)
   fei::DevBuf aux[FEI_MAX_AUX]; uint64_t aux_n[FEI_MAX_AUX] = {0};   // host-computed per-record verdict bytes (fei_corpus_set_aux, FEI_C_RECBITS)
-  fei::DevBuf stage_raw, stage_raw_off, stage_ms, stage_hlen, stage_blen;   // raw ingest staging (ingest.cu)
+  fei::DevBuf stage_raw, stage_raw_off, stage_raw_len, stage_ms, stage_hlen, stage_blen;   // raw ingest staging (ingest.cu)
   // scan scratch (grown on demand, reused across scans)
   fei::DevBuf prog, hits, hit_lists, work_counter, scan_tmp, survivors, live_list, win_done, win_state;
   fei::CompactScratch compact;
@@ -81,10 +96,16 @@ struct fei_corpus {
 };
 
 namespace fei {
-// builds tiles from a canonical body blob already on the device (body has >= 32 bytes of slack)
 int corpus_load_events(fei_corpus* c);              // ev_load[], created on first use
 cudaStream_t corpus_load_stream(fei_corpus* c);   // created on first use; falls back to the context's copy stream
-int build_tiles(fei_corpus* c, const uint8_t* d_body, const uint64_t* d_body_off, cudaStream_t s);
+// Checks every load makes before it touches the handle (caller holds c->mu): the device is bound, n fits the tiles' 32-bit
+// record indices and, when h is given, the meta arrays are there.
+int check_load(uint64_t n, const fei_corpus_host* h);
+// ts / wall / flags8 / fsb and the optional names of h, queued on s
+int upload_meta(fei_corpus* c, const fei_corpus_host* h, cudaStream_t s);
+// The end of every load: tiles from the canonical body on the device (kBlobSlack zeroed bytes behind it), then the header
+// directory from hdr / hdr_off, then `loaded`.  `packed` (may be null) is recorded after the pack kernels.
+int pack_canonical(fei_corpus* c, DevBuf& body, DevBuf& body_off, cudaStream_t s, bool drop_text, cudaEvent_t packed);
 // builds the header directory from hdr / hdr_off already on the device (hdir.cu)
 int build_header_dir(fei_corpus* c, cudaStream_t s);
 int exclusive_scan_u32_u64(const uint32_t* in, uint64_t n, uint64_t* out, DevBuf& tmp, cudaStream_t s);

@@ -83,14 +83,6 @@ __global__ void __launch_bounds__(256) k_hdir(const uint8_t* __restrict__ hdr, c
 }
 
 // ---------------------------------------------------------------- value columns
-__device__ __forceinline__ uint4 load16_any(const uint8_t* s) {          // 16 bytes from any address (>= 32 bytes of slack behind the blob)
-  const uintptr_t a = reinterpret_cast<uintptr_t>(s);
-  const uint32_t* w = reinterpret_cast<const uint32_t*>(a & ~uintptr_t(3));
-  const uint32_t sh = (uint32_t)(a & 3) * 8;
-  const uint32_t w0 = w[0], w1 = w[1], w2 = w[2], w3 = w[3], w4 = sh ? w[4] : 0;
-  return make_uint4(__funnelshift_r(w0, w1, sh), __funnelshift_r(w1, w2, sh), __funnelshift_r(w2, w3, sh), __funnelshift_r(w3, w4, sh));
-}
-
 // Thread per record: for every directory entry whose key has a column, store the value (the last line with that key wins,
 // like the dict assignment of utils.py:118) as 16-byte units in the column's planes.
 __global__ void __launch_bounds__(256) k_hdir_cols(const uint8_t* __restrict__ hdr, const uint64_t* __restrict__ hdr_off, uint64_t n,
@@ -115,7 +107,7 @@ __global__ void __launch_bounds__(256) k_hdir_cols(const uint8_t* __restrict__ h
     col_len[(uint64_t)c * n + i] = (uint16_t)len;
     uint8_t* base = planes + (uint64_t)c * kColUnits * n * 16 + i * 16;
     for (uint32_t k = 0; k * 16 < len; ++k)
-      *reinterpret_cast<uint4*>(base + (uint64_t)k * n * 16) = load16_any(h + e.y + k * 16);     // bytes past `len` are never looked at
+      *reinterpret_cast<uint4*>(base + (uint64_t)k * n * 16) = load16(h + e.y + k * 16);     // bytes past `len` are never looked at
   }
 }
 

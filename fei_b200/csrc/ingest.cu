@@ -254,13 +254,10 @@ using namespace fei;
 // undecodable ones (and print the reference's message) and call again with the survivors.
 static int load_raw_impl(fei_corpus* c, const fei_corpus_host* h, const uint8_t* raw, uint64_t raw_bytes_in, const uint64_t* raw_off,
                          const uint64_t* raw_len, uint8_t* valid_out) {
-  if (!c) { set_error("null corpus"); return FEI_E_BADARG; }
-  std::lock_guard<std::mutex> lock(c->mu);
-  FEI_TRY(require_ready());
   if (!c || !h || !raw_off) { set_error("null argument"); return FEI_E_BADARG; }
+  std::lock_guard<std::mutex> lock(c->mu);
+  FEI_TRY(check_load(h->n, h));
   const bool staged = h->n && !raw;                                     // raw == NULL: the text was put on the device by fei_corpus_stage_text
-  if (h->n >= 0xFFFFFFFFull) { set_error("at most 2^32-2 records per shard"); return FEI_E_BADARG; }
-  if (h->n && (!h->ts || !h->wall || !h->flags8 || !h->fsb)) { set_error("missing meta array"); return FEI_E_BADARG; }
   // loads run on the copy stream: a batch can be uploaded / normalised / tiled into one handle while another handle is being
   // scanned on the compute stream (streaming e2e use); the staging buffers live in the handle (grow-only) because a
   // cudaFree in the middle of a pipeline synchronises the whole device
@@ -278,29 +275,15 @@ static int load_raw_impl(fei_corpus* c, const fei_corpus_host* h, const uint8_t*
   }
   FEI_TRY(corpus_load_events(c));
   DevBuf& d_raw = c->stage_raw; DevBuf& d_raw_off = c->stage_raw_off; DevBuf& d_ms = c->stage_ms; DevBuf& d_hlen = c->stage_hlen; DevBuf& d_blen = c->stage_blen;
-  FEI_TRY(d_raw.ensure(raw_bytes + 64)); FEI_TRY(d_raw_off.ensure((n + 1) * 8 * (raw_len ? 2 : 1)));
+  FEI_TRY(d_raw.ensure(raw_bytes + 64));
   FEI_TRY(d_ms.ensure((n ? n : 1) * sizeof(RawMeasure) + 16)); FEI_TRY(d_hlen.ensure((n ? n : 1) * 4)); FEI_TRY(d_blen.ensure((n ? n : 1) * 4));
   // The small host arrays go first: a second handle's multi-GB text copy may already sit in the copy engine's queue when this load
   // reaches its tail, and anything this load still had to upload then would wait behind it (and the next load behind this one).
   // meta columns + names come from the host (file-name grammar and listing order stay there)
-  auto up = [&](DevBuf& b, const void* src, size_t bytes) -> int {
-    FEI_TRY(b.ensure(bytes + 16));
-    if (bytes) FEI_CUDA(cudaMemcpyAsync(b.p, src, bytes, cudaMemcpyHostToDevice, s));
-    return FEI_OK;
-  };
-  FEI_TRY(up(c->ts, h->ts, n * 8)); FEI_TRY(up(c->wall, h->wall, n * 8)); FEI_TRY(up(c->flags8, h->flags8, n * 8)); FEI_TRY(up(c->fsb, h->fsb, n * 4));
-  if (h->name && h->name_off && h->name_spans && n) {
-    c->name_bytes = h->name_off[n];
-    FEI_TRY(up(c->name, h->name, c->name_bytes)); FEI_TRY(up(c->name_off, h->name_off, (n + 1) * 8)); FEI_TRY(up(c->name_spans, h->name_spans, n * 8));
-  } else { c->name.release(); c->name_off.release(); c->name_spans.release(); c->name_bytes = 0; }
-  const uint64_t* d_len = nullptr;
-  if (raw_len) {                                                        // spans: n begins, then n lengths
-    if (n) FEI_CUDA(cudaMemcpyAsync(d_raw_off.p, raw_off, n * 8, cudaMemcpyHostToDevice, s));
-    if (n) FEI_CUDA(cudaMemcpyAsync(d_raw_off.as<uint64_t>() + n + 1, raw_len, n * 8, cudaMemcpyHostToDevice, s));
-    d_len = d_raw_off.as<uint64_t>() + n + 1;
-  } else {
-    FEI_CUDA(cudaMemcpyAsync(d_raw_off.p, raw_off, (n + 1) * 8, cudaMemcpyHostToDevice, s));
-  }
+  FEI_TRY(upload_meta(c, h, s));
+  FEI_TRY(upload(d_raw_off, raw_off, (raw_len ? n : n + 1) * 8, 0, s));      // spans: n begins and n lengths; else n + 1 offsets
+  if (raw_len) FEI_TRY(upload(c->stage_raw_len, raw_len, n * 8, 0, s));
+  const uint64_t* d_len = raw_len ? c->stage_raw_len.as<uint64_t>() : nullptr;
   FEI_CUDA(cudaEventRecord(c->ev_load[0], s));
   // in pieces at fixed offsets: the host buffer may be page-locked block by block (the packer's arena: a copy must not straddle two
   // registrations), and a failed registration leaves one block pageable without slowing the others
@@ -341,18 +324,14 @@ static int load_raw_impl(fei_corpus* c, const fei_corpus_host* h, const uint8_t*
   if (summary[1]) { set_error("record %llu: body larger than 32 MiB is not supported", summary[1] - 1ull); return FEI_E_UNSUPPORTED; }
   c->n = n; c->global_base = h->global_base;
   c->hdr_bytes = hb; c->body_bytes = bb;
-  FEI_TRY(c->hdr.ensure(hb + 64)); FEI_TRY(body.ensure(bb + 64));
-  FEI_CUDA(cudaMemsetAsync((uint8_t*)c->hdr.p + hb, 0, 48, s));
-  FEI_CUDA(cudaMemsetAsync((uint8_t*)body.p + bb, 0, 48, s));
+  FEI_TRY(c->hdr.ensure(hb + kBlobSlack)); FEI_TRY(body.ensure(bb + kBlobSlack));
+  FEI_CUDA(cudaMemsetAsync((uint8_t*)c->hdr.p + hb, 0, kBlobSlack, s));
+  FEI_CUDA(cudaMemsetAsync((uint8_t*)body.p + bb, 0, kBlobSlack, s));
   if (n) k_raw_write<<<gw, kIngestThreads, 0, s>>>(d_raw.as<uint8_t>(), d_raw_off.as<uint64_t>(), d_len, n, d_ms.as<RawMeasure>(), c->hdr_off.as<uint64_t>(), body_off.as<uint64_t>(),
                                        c->hdr.as<uint8_t>(), body.as<uint8_t>());
   if (n) k_fix_fsb<<<g, 128, 0, s>>>(d_ms.as<RawMeasure>(), n, c->fsb.as<uint32_t>());
   FEI_CUDA(cudaGetLastError());
-  FEI_TRY(build_tiles(c, body.as<uint8_t>(), body_off.as<uint64_t>(), s));
-  FEI_TRY(build_header_dir(c, s));
-  FEI_CUDA(cudaEventRecord(c->ev_load[2], s));
-  if (body.bytes > (8ull << 30)) { body.release(); body_off.release(); c->tmp_len.release(); c->tmp_gunits.release(); d_raw.release(); c->staged_text_bytes = ~0ull; }
-  c->loaded = true;
+  FEI_TRY(pack_canonical(c, body, body_off, s, false, c->ev_load[2]));
   c->load_timed = true;
   return FEI_OK;
 }

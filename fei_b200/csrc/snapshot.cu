@@ -2,7 +2,6 @@
 // dictionary, value columns) written to / restored from one file, so that a process restart does not re-walk and re-pack the
 // Memdir tree (the reference re-reads every file on every query, memdir_tools/utils.py:202-253).  Restoring streams the file
 // through a ring of pinned buffers: reader threads pread the next chunks while the copy engine uploads the previous ones.
-// Also here: fetch of arbitrary records by index (materialising hits without keeping any file content on the host).
 #include "corpus.h"
 #include <fcntl.h>
 #include <unistd.h>
@@ -166,89 +165,5 @@ extern "C" int fei_corpus_load_snapshot(fei_corpus* c, const char* path, float* 
   for (int x = 0; x < FEI_MAX_AUX; ++x) { c->aux[x].release(); c->aux_n[x] = 0; }
   c->loaded = true;
   if (gbs_out) *gbs_out = ms > 0 ? (float)((double)total_bytes / 1e9 / (ms * 1e-3)) : 0.f;
-  return FEI_OK;
-}
-
-// ---------------------------------------------------------------- fetch by index
-namespace fei {
-__global__ void k_rec_lens(const uint64_t* __restrict__ idx, uint64_t m, const uint64_t* __restrict__ hdr_off, const uint32_t* __restrict__ rec_pos,
-                           const uint32_t* __restrict__ grp_len, uint32_t* __restrict__ hlen, uint32_t* __restrict__ blen) {
-  const uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
-  if (i >= m) return;
-  const uint64_t r = idx[i];
-  hlen[i] = (uint32_t)(hdr_off[r + 1] - hdr_off[r]);
-  blen[i] = grp_len[rec_pos[r]];
-}
-__global__ void k_copy_hdr(const uint64_t* __restrict__ idx, uint64_t m, const uint8_t* __restrict__ hdr, const uint64_t* __restrict__ hdr_off,
-                           const uint64_t* __restrict__ out_off, uint8_t* __restrict__ out) {
-  const uint64_t i = (blockIdx.x * (uint64_t)blockDim.x + threadIdx.x) >> 5;       // a warp per record
-  const int lane = threadIdx.x & 31;
-  if (i >= m) return;
-  const uint64_t r = idx[i];
-  const uint8_t* p = hdr + hdr_off[r];
-  const uint32_t len = (uint32_t)(hdr_off[r + 1] - hdr_off[r]);
-  uint8_t* d = out + out_off[i];
-  for (uint32_t k = lane; k < len; k += 32) d[k] = p[k];
-}
-__global__ void k_untile_idx(const uint8_t* __restrict__ tiles, const uint64_t* __restrict__ grp_base, const uint32_t* __restrict__ grp_len,
-                             const uint32_t* __restrict__ rec_pos, const uint64_t* __restrict__ idx, uint64_t m,
-                             const uint64_t* __restrict__ out_off, uint8_t* __restrict__ out) {
-  const uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
-  if (i >= m) return;
-  const uint32_t pos = rec_pos[idx[i]];
-  const uint64_t g = pos >> 5; const int lane = pos & 31;
-  const uint32_t len = grp_len[pos];
-  const uint32_t* gl = grp_len + g * 32;
-  uint8_t* dst = out + out_off[i];
-  const uint8_t* gb = tiles + grp_base[g] * 16;
-  uint32_t units[32];
-  for (int l = 0; l < 32; ++l) units[l] = (gl[l] + 15) >> 4;
-  for (uint32_t k = 0; k * 16 < len; ++k) {
-    uint64_t before = 0;
-    for (int l = 0; l < 32; ++l) before += units[l] < k ? units[l] : k;
-    const uint8_t* p = gb + before * 16 + lane * 16;
-    const uint32_t cnt = len - k * 16 < 16 ? len - k * 16 : 16;
-    for (uint32_t b = 0; b < cnt; ++b) { const uint8_t t = p[b]; dst[k * 16 + b] = (uint8_t)(t ^ ((t >> 1) & 0x20)); }
-  }
-}
-}  // namespace fei
-
-/* Header text and body of the m records idx[0..m) (any order, repeats allowed), for materialising hits: hdr_off / body_off get
- * m + 1 offsets; FEI_E_CAPACITY (needed sizes in hdr_off[m] / body_off[m]) when a blob is too small.  hdr / body may be NULL to
- * only size the buffers.                                                                                                         */
-extern "C" int fei_corpus_fetch_records(fei_corpus* c, const uint64_t* idx, uint64_t m, uint8_t* hdr, uint64_t hdr_cap, uint64_t* hdr_off,
-                                        uint8_t* body, uint64_t body_cap, uint64_t* body_off) {
-  if (!c || (m && !idx) || !hdr_off || !body_off) { set_error("null argument"); return FEI_E_BADARG; }
-  std::lock_guard<std::mutex> lock(c->mu);
-  FEI_TRY(require_ready());
-  if (!c->loaded) { set_error("corpus not loaded"); return FEI_E_STATE; }
-  hdr_off[0] = 0; body_off[0] = 0;
-  if (m == 0) return FEI_OK;
-  for (uint64_t i = 0; i < m; ++i) if (idx[i] >= c->n) { set_error("record index %llu out of range", (unsigned long long)idx[i]); return FEI_E_BADARG; }
-  cudaStream_t s = ctx().stream;
-  DevBuf d_idx, d_hlen, d_blen, d_hoff, d_boff, d_h, d_b;
-  FEI_TRY(d_idx.alloc(m * 8)); FEI_TRY(d_hlen.alloc(m * 4)); FEI_TRY(d_blen.alloc(m * 4)); FEI_TRY(d_hoff.alloc((m + 1) * 8)); FEI_TRY(d_boff.alloc((m + 1) * 8));
-  FEI_CUDA(cudaMemcpyAsync(d_idx.p, idx, m * 8, cudaMemcpyHostToDevice, s));
-  const unsigned grid = (unsigned)((m + 127) / 128);
-  k_rec_lens<<<grid, 128, 0, s>>>(d_idx.as<uint64_t>(), m, c->hdr_off.as<uint64_t>(), c->rec_pos.as<uint32_t>(), c->grp_len.as<uint32_t>(), d_hlen.as<uint32_t>(), d_blen.as<uint32_t>());
-  FEI_TRY(exclusive_scan_u32_u64(d_hlen.as<uint32_t>(), m, d_hoff.as<uint64_t>(), c->scan_tmp, s));
-  FEI_TRY(exclusive_scan_u32_u64(d_blen.as<uint32_t>(), m, d_boff.as<uint64_t>(), c->scan_tmp, s));
-  FEI_CUDA(cudaMemcpyAsync(hdr_off, d_hoff.p, (m + 1) * 8, cudaMemcpyDeviceToHost, s));
-  FEI_CUDA(cudaMemcpyAsync(body_off, d_boff.p, (m + 1) * 8, cudaMemcpyDeviceToHost, s));
-  FEI_CUDA(cudaStreamSynchronize(s));
-  if ((hdr && hdr_off[m] > hdr_cap) || (body && body_off[m] > body_cap)) { set_error("fetch buffers too small: need %llu header and %llu body bytes", (unsigned long long)hdr_off[m], (unsigned long long)body_off[m]); return FEI_E_CAPACITY; }
-  if (hdr && hdr_off[m]) {
-    FEI_TRY(d_h.alloc(hdr_off[m] + 16));
-    k_copy_hdr<<<(unsigned)((m * 32 + 255) / 256), 256, 0, s>>>(d_idx.as<uint64_t>(), m, c->hdr.as<uint8_t>(), c->hdr_off.as<uint64_t>(), d_hoff.as<uint64_t>(), d_h.as<uint8_t>());
-    FEI_CUDA(cudaMemcpyAsync(hdr, d_h.p, hdr_off[m], cudaMemcpyDeviceToHost, s));
-  }
-  if (body && body_off[m]) {
-    FEI_TRY(d_b.alloc(body_off[m] + 16));
-    k_untile_idx<<<grid, 128, 0, s>>>(c->tiles.as<uint8_t>(), c->grp_base.as<uint64_t>(), c->grp_len.as<uint32_t>(), c->rec_pos.as<uint32_t>(), d_idx.as<uint64_t>(), m,
-                                      d_boff.as<uint64_t>(), d_b.as<uint8_t>());
-    FEI_CUDA(cudaMemcpyAsync(body, d_b.p, body_off[m], cudaMemcpyDeviceToHost, s));
-  }
-  FEI_CUDA(cudaStreamSynchronize(s));
-  FEI_CUDA(cudaGetLastError());
   return FEI_OK;
 }
