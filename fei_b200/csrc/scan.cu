@@ -805,6 +805,11 @@ __device__ __forceinline__ uint32_t shl_clamp(uint32_t v, uint32_t n) {   // PTX
   return r;
 }
 
+// The size of a table entry as a value ptxas cannot see.  With the immediate 2 it turns column * 2 + trans_s into LEA, an
+// ALU-pipe instruction like PRMT, SHF and LOP3; with a register operand the multiply-add stays IMAD on the FMA pipe.
+// That is 16 of 93 ALU-pipe instructions per row of k_body<direct, acc64> (DESIGN 5.1).
+__constant__ uint32_t c_entry_bytes = 2;
+
 // One DFA step.  kAcc selects how accepting states are recorded (they are numbered 0..n_acc-1):
 //   1 / 2 : branch-free, bit k of (a0,a1) = "accepting state k was visited" (n_acc <= 32 / <= 64):
 //           no second shared-memory lookup and no divergent branch in the byte loop; the pattern
@@ -817,12 +822,14 @@ struct BodyDfa {
   uint32_t trans_s;            // shared-space address of the transition table
   const uint32_t* out; const uint8_t* cls;
   uint32_t stride2, n_acc;     // stride2 = row stride in bytes
+  uint32_t entry_bytes;        // c_entry_bytes in a register
   uint32_t s, a0;
   unsigned long long a64;
   __device__ __forceinline__ void step(uint32_t b) {
     uint32_t col = kDirect ? b : cls[b];
     uint32_t t, addr;
-    asm("mad.lo.u32 %0, %1, 2, %2;" : "=r"(t) : "r"(col), "r"(trans_s));        // IMAD (FMA pipe)
+    if (kAcc == 3) asm("mad.lo.u32 %0, %1, 2, %2;" : "=r"(t) : "r"(col), "r"(trans_s));
+    else asm("mad.lo.u32 %0, %1, %2, %3;" : "=r"(t) : "r"(col), "r"(entry_bytes), "r"(trans_s));   // IMAD (FMA pipe)
     asm("mad.lo.u32 %0, %1, %2, %3;" : "=r"(addr) : "r"(s), "r"(stride2), "r"(t));
     uint16_t nxt;
     asm volatile("ld.shared.u16 %0, [%1];" : "=h"(nxt) : "r"(addr));
@@ -941,7 +948,7 @@ __global__ void __launch_bounds__(kBodyThreads, 1) k_body(BodyArgs a) {
   d.trans_s = smem_u32(smem);
   d.out = reinterpret_cast<const uint32_t*>(smem + (dd->off_out - dd->off_trans));
   d.cls = smem + (dd->off_cls - dd->off_trans);
-  d.stride2 = dd->row_stride * 2u; d.n_acc = dd->n_acc;
+  d.stride2 = dd->row_stride * 2u; d.n_acc = dd->n_acc; d.entry_bytes = c_entry_bytes;
   const uint32_t sticky_state = dd->sticky ? dd->sticky - 1u : 0xFFFFFFFFu;
 
   for (;;) {
@@ -962,6 +969,9 @@ __global__ void __launch_bounds__(kBodyThreads, 1) k_body(BodyArgs a) {
     }
     const uint8_t* row = a.tiles + a.grp_base[g] * 16;
     const uint32_t maxu = __shfl_sync(0xffffffffu, units, 0);
+    // rows below plain_end hold 16 bytes of every one of the 32 records: 512 bytes each, no partial row
+    const uint32_t minu = kAcc == 3 ? 0u : __reduce_min_sync(0xffffffffu, units);
+    const uint32_t plain_end = minu ? minu - 1u : 0u;
     if (lane == 0) touched += (a.grp_base[g + 1] - a.grp_base[g]) * 16;
     d.reset(start);
     // lim: rows this lane steps through; units, or fewer once its verdicts are decided (0: not live, or decided at the start)
@@ -981,6 +991,29 @@ __global__ void __launch_bounds__(kBodyThreads, 1) k_body(BodyArgs a) {
     for (uint32_t k0 = 0; k0 < maxu;) {
       const uint32_t k1 = kAcc == 3 || maxu - k0 <= kDecideRows ? maxu : k0 + kDecideRows;
       bool stop = false;
+      // The block's plain rows, without the per-row lane count, 64-bit row step and partial-row test of the loop below.  A lane
+      // runs all of them or none: lim is its units, or a block boundary where it was decided.  The test of k against lim inside
+      // the loop is always true; it ends the basic block after the load, which ptxas otherwise sinks below the row's tenth
+      // lookup, and a load issued that late arrives late (DESIGN 5.1).  The row four ahead is asked into L2 meanwhile.
+      if constexpr (kAcc != 3) {
+        const uint32_t kp = k1 < plain_end ? k1 : plain_end;
+        if (k0 < kp) {
+          if (k0 < lim) {
+            const uint8_t* p = row + lane * 16;
+#pragma unroll 1
+            for (uint32_t k = k0; k < kp; ++k) {
+              p += 512;
+              const uint4 nxt = ldg_stream16(p);
+              if (k + 4 < minu) asm volatile("prefetch.global.L2 [%0];" :: "l"(p + 3 * 512));
+              if (k < lim) { d.word(cur.x); d.word(cur.y); d.word(cur.z); d.word(cur.w); }
+              cur = nxt;
+            }
+            rows_read += kp - k0;
+          }
+          row += (uint64_t)(kp - k0) * 512;
+          k0 = kp;
+        }
+      }
       for (uint32_t k = k0; k < k1; ++k) {
         const uint32_t m = __popc(__ballot_sync(0xffffffffu, k < units));
         const uint8_t* next_row = row + (uint64_t)m * 16;
