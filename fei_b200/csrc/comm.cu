@@ -36,7 +36,7 @@ struct Nccl {
   const char* (*GetErrorString)(int) = nullptr;
   ncclComm_t comm = nullptr;
   int nranks = 0, rank = -1;
-  DevBuf counts_dev, gathered, scratch, lists;
+  DevBuf counts_dev, gathered, gathered_local, scratch, lists;
   CompactScratch compact;
   std::mutex mu;                 // one collective at a time per communicator
   // ---- bound shard set (fei_comm_bind_corpus): record count / first global index of every rank's shard, the rank-major
@@ -288,7 +288,7 @@ extern "C" int fei_comm_init(const uint8_t* id, int nranks, int rank) {
 extern "C" int fei_comm_destroy(void) {
   if (g.comm) { g.CommDestroy(g.comm); g.comm = nullptr; }
   unbind();
-  g.counts_dev.release(); g.gathered.release(); g.scratch.release(); g.lists.release(); g.gathered_masks.release(); g.totals_dev.release(); g.global_lists.release();
+  g.counts_dev.release(); g.gathered.release(); g.gathered_local.release(); g.scratch.release(); g.lists.release(); g.gathered_masks.release(); g.totals_dev.release(); g.global_lists.release();
   if (g.totals_host) { cudaFreeHost(g.totals_host); g.totals_host = nullptr; }
   g.last_kind = 0;
   g.compact.blk_counts.release(); g.compact.blk_offsets.release(); g.compact.totals.release();
@@ -297,8 +297,9 @@ extern "C" int fei_comm_destroy(void) {
 }
 
 // All-gatherv of the scan result of every rank.  Two wire formats, chosen per call from the gathered counts:
-//   sparse : the compacted per-query index lists (8 B per hit), one grouped ncclBroadcast per (rank, query)
-//            segment straight into its final position;
+//   sparse : the compacted per-query index lists, one grouped ncclBroadcast per (rank, query) segment of the
+//            rank's corpus-local 32-bit entries (4 B per hit) straight into its final position, then widened on
+//            the receiver with that rank's global_base into the 64-bit global lists;
 //   dense  : when the lists would be larger than the per-record hit masks (4 B per record) — typical for
 //            many-pattern batches where most records hit — the masks are all-gathered instead (one
 //            ncclAllGather) and the global ordered lists are compacted from them on demand.
@@ -343,19 +344,28 @@ extern "C" int fei_comm_allgather_hits(fei_corpus* c, uint32_t nq, uint64_t* con
     for (uint32_t q = 0; q < nq; ++q) qbase[q + 1] = qbase[q] + tot[q];
     for (uint32_t q = 0; q <= nq; ++q) g.last_qbase[q] = qbase[q];
     FEI_TRY(g.gathered.ensure((qbase[nq] + 1) * sizeof(uint64_t)));
+    FEI_TRY(g.gathered_local.ensure((qbase[nq] + 1) * sizeof(uint32_t)));
     FEI_NCCL(g.GroupStart());
     for (uint32_t q = 0; q < nq; ++q) {
       uint64_t pos = qbase[q];
       for (int r = 0; r < R; ++r) {
         uint64_t cnt = info[(size_t)r * W + q];
         if (cnt) {
-          const void* src = c->hit_lists.as<uint64_t>() + (size_t)q * c->hit_list_stride;   // only read on the root
-          FEI_NCCL(g.Broadcast(src, g.gathered.as<uint64_t>() + pos, cnt, ncclUint64, r, g.comm, s));
+          const void* src = c->hit_lists.as<uint32_t>() + (size_t)q * c->hit_list_stride;   // only read on the root
+          FEI_NCCL(g.Broadcast(src, g.gathered_local.as<uint32_t>() + pos, cnt, ncclUint32, r, g.comm, s));
         }
         pos += cnt;
       }
     }
     FEI_NCCL(g.GroupEnd());
+    for (uint32_t q = 0; q < nq; ++q) {
+      uint64_t pos = qbase[q];
+      for (int r = 0; r < R; ++r) {
+        const uint64_t cnt = info[(size_t)r * W + q];
+        FEI_TRY(widen_list(g.gathered_local.as<uint32_t>() + pos, cnt, g.last_base[r], g.gathered.as<uint64_t>() + pos, s));
+        pos += cnt;
+      }
+    }
     for (uint32_t q = 0; want_host && q < nq; ++q) {
       if (!hits[q]) continue;
       uint64_t take = tot[q] < cap[q] ? tot[q] : cap[q];

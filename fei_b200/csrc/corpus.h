@@ -83,8 +83,11 @@ struct fei_corpus {
   fei::DevBuf stage_raw, stage_raw_off, stage_raw_len, stage_ms, stage_hlen, stage_blen;   // raw ingest staging (ingest.cu)
   // scan scratch (grown on demand, reused across scans)
   fei::DevBuf prog, hits, hit_lists, work_counter, scan_tmp, survivors, live_list, win_done, win_state;
+  fei::DevBuf list_stage;                // one list widened to global indices on its way to the host (fei_scan_hits / fei_scan_fetch_hits)
   fei::CompactScratch compact;
-  uint64_t hit_list_stride = 0;          // entries per query in hit_lists (last fei_scan_hits)
+  // hit_lists: the ordered lists of the last list-building scan, query q at q * hit_list_stride, as corpus-local 32-bit record
+  // indices (global index = global_base + entry; the C ABI hands out global ones)
+  uint64_t hit_list_stride = 0;          // entries per query in hit_lists
   uint32_t last_nq = 0;
   uint64_t last_counts[32] = {0};
   fei_scan_timing timing = {};
@@ -125,7 +128,11 @@ int run_scan(fei_corpus* c, const uint8_t* prog, uint64_t prog_len, int compact_
 int finish_timing(fei_corpus* c, bool compacted);
 int compact_segments(const uint32_t* masks, uint64_t seg_stride, const uint64_t* seg_n, const uint64_t* seg_base, uint32_t n_seg, uint32_t nq,
                      CompactScratch& sc, uint64_t stride, uint64_t* lists, uint64_t* totals_out, cudaStream_t s);
+// (A, S) checksums of a list of global indices, or of a corpus-local one (index = base + entry); see k_list_checksum
 int list_checksum(const uint64_t* list, uint64_t count, DevBuf& tmp, uint64_t* a_out, uint64_t* s_out, cudaStream_t s);
+int list_checksum(const uint32_t* list, uint64_t count, uint64_t base, DevBuf& tmp, uint64_t* a_out, uint64_t* s_out, cudaStream_t s);
+// dst[i] = base + src[i] for i < n, queued on s
+int widen_list(const uint32_t* src, uint64_t n, uint64_t base, uint64_t* dst, cudaStream_t s);
 int compact_masks(const uint32_t* masks, uint64_t n, uint32_t nq, uint64_t global_base, CompactScratch& sc,
                   uint64_t* counts_out, DevBuf* lists, uint64_t* stride_out, uint32_t* launches, cudaStream_t s);
 }

@@ -20,12 +20,13 @@
 //          its own record through the multi-pattern DFA whose tables were staged into shared
 //          memory with 1-D TMA bulk copies (cp.async.bulk + mbarrier).  Groups with no live
 //          record are skipped without touching their bytes.  hits[i] = alive[i] & content bits.
-//          The warp that completes a window of 4096 records also appends the window's hits to the
-//          per-query ordered lists (build_window_lists: decoupled look-back over the windows); warps
-//          with no group left help write the last windows' lists (help_tail).
+//          In a list-building scan every warp stores its group's per-query hit counts (store_group_counts),
+//          and the warp that completes a window of 4096 records adds them up and appends the window's hits
+//          to the per-query ordered lists of 32-bit corpus-local indices (build_window_lists: decoupled
+//          look-back over the windows); warps with no group left help write the last windows' lists (help_tail).
 // k_count / k_scan_blocks / k_emit : order-preserving compaction of hits[] into per-query lists
-//          of global record indices (warp ballots + popc prefix, block offsets from a scan), for
-//          the single-pattern kernels, header-only programs and gathered multi-GPU masks.
+//          (warp ballots + popc prefix, block offsets from a scan): corpus-local 32-bit indices for the
+//          single-pattern kernels and header-only programs, 64-bit global ones for gathered multi-GPU masks.
 #include "corpus.h"
 #include "../../include/feiscan_prog.h"
 #include "pyws.cuh"
@@ -580,8 +581,9 @@ struct BodyArgs {
   // make ptxas copy it to local memory).
   uint32_t* const* push_peers; uint32_t push_n; unsigned long long push_off, n_records;
   // ordered hit lists (k_body): the warp that completes a window also writes the window's part of every query's list
-  // (build_window_lists); win_state holds kWinBytes of look-back / emit state per window, zeroed once per scan
-  uint64_t* lists; unsigned long long list_stride, list_base;
+  // (build_window_lists); win_state holds kWinBytes of look-back / count / emit state per window, zeroed once per scan.
+  // List entries are corpus-local record indices (32-bit, like grp_rec).
+  uint32_t* lists; unsigned long long list_stride;
   unsigned long long* totals; uint8_t* win_state; uint32_t nq;
 };
 constexpr uint32_t kGroupsPerWindow = kWindow / 32;
@@ -617,28 +619,28 @@ __device__ __forceinline__ uint32_t count_hits32(uint32_t m, uint32_t nq, int la
   }
   return cnt;
 }
-// query q of the warp's 32 masks in lane order: a lane whose mask has bit q stores `rec` (its global index) at
-// lists[q * stride + pos + hits of the lanes below it]; returns the warp's hits of query q
-__device__ __forceinline__ uint32_t emit_hits32(uint32_t m, uint32_t q, uint64_t pos, uint64_t rec, uint64_t stride, uint64_t* lists, int lane) {
-  const bool hit = (m >> q) & 1u;
+// one query over the warp's 32 records in lane order: a lane with `hit` stores `rec` at list[hits of the lanes below it]
+// (the caller points `list` at the rank of the warp's first hit); returns the warp's hits
+template <class T>
+__device__ __forceinline__ uint32_t emit_hits32(bool hit, T* list, T rec, int lane) {
   const uint32_t bal = __ballot_sync(0xffffffffu, hit);
-  if (hit) {
-    const uint64_t rank = pos + __popc(bal & ((1u << lane) - 1u));
-    if (rank < stride) __stcs(reinterpret_cast<unsigned long long*>(lists + q * stride + rank), (unsigned long long)rec);   // nothing reads them back soon
-  }
+  if (hit) __stcs(list + __popc(bal & ((1u << lane) - 1u)), rec);       // nothing reads them back soon
   return __popc(bal);
 }
 
 // Per-window state of the list building, one record of kWinBytes per window, zeroed once per scan:
 //   desc[32]  look-back descriptor of (window, query): flag in the top 2 bits over a 62-bit hit count;
-//   ready     set (release) once excl[] and boff[] below are written;   claim: blocks of the window's emit handed out so far;
-//   excl[32]  hits of query q in all earlier windows;   boff[b][32]: hits of query q in the window's records before block b.
-// The emit of a window is cut into kEmitBlocks blocks of kEmitBlockRecs records, claimed one at a time: the completer of the
-// window takes them, and so do warps that find no group left to scan (help_tail), so the last windows' lists are written by
-// many warps instead of one each after the scan ends.
+//   ready     set (release) once excl[] below is written;   claim: query slices of the window's emit handed out so far;
+//   excl[32]  hits of query q in all earlier windows;
+//   cnt[128]  one 32-byte row per group of the window (store_group_counts): byte 4k + j = the group's hits of query 8j + k.
+// The emit of a window is cut into slices of kEmitQueries queries, claimed one at a time: the completer of the window takes
+// them, and so do warps that find no group left to scan (help_tail), so the last windows' lists are written by many warps
+// instead of one each after the scan.  A slice spans the whole window: the length sort spreads the records of a group over
+// the window, so the group counts give per-query window totals but not the offsets of record ranges inside it.
 constexpr unsigned long long kDescAggregate = 1ull << 62, kDescPrefix = 2ull << 62, kDescCount = (1ull << 62) - 1;
-constexpr uint32_t kEmitBlocks = 16, kEmitBlockRecs = kWindow / kEmitBlocks;
-constexpr uint32_t kWinDesc = 0, kWinCtl = 256, kWinExcl = 272, kWinBoff = 528, kWinBytes = kWinBoff + kEmitBlocks * 32 * 4;
+constexpr uint32_t kEmitQueries = 2, kEmitRows = 4;  // queries per claimed slice; rows of 32 masks loaded at once
+constexpr uint32_t kWinDesc = 0, kWinCtl = 256, kWinExcl = 272, kWinCnt = 528, kWinBytes = kWinCnt + kGroupsPerWindow * 32;
+static_assert(kWinCnt % 16 == 0 && kWinBytes % 16 == 0, "count rows are stored 16 bytes at a time");
 constexpr uint32_t kHelpWindows = 64;              // windows at the end of the scan that warps without a group help with
 __device__ __forceinline__ void st_release_u64(unsigned long long* p, unsigned long long v) {
   asm volatile("st.release.gpu.global.u64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
@@ -657,73 +659,90 @@ __device__ __forceinline__ unsigned int ld_acquire_u32(const unsigned int* p) {
   return v;
 }
 
-// Claims blocks of window w's emit until none is left and writes each block's hits in record order (the window is ready).
-__device__ __forceinline__ void emit_claimed(const uint32_t* __restrict__ hits, uint8_t* __restrict__ win, uint64_t* __restrict__ lists,
-                                             unsigned long long stride, unsigned long long list_base, unsigned long long n_records,
-                                             uint32_t nq, unsigned long long w, int lane) {
+// The hits per query of group g, from the 32 masks its scanning warp still holds (0 in lanes without a record), into the
+// group's count row of its window: byte j of sum k counts query 8j + k (at most 32, so no carry into the next byte).  Out of
+// line, like build_window_lists: the row loop of k_body keeps its register allocation.
+__device__ __noinline__ void store_group_counts(uint8_t* __restrict__ win, unsigned long long g, uint32_t m, int lane) {
+  uint32_t c[8];
+#pragma unroll
+  for (int k = 0; k < 8; ++k) c[k] = __reduce_add_sync(0xffffffffu, (m >> k) & 0x01010101u);
+  if (lane == 0) {
+    uint4* row = reinterpret_cast<uint4*>(win + (g / kGroupsPerWindow) * kWinBytes + kWinCnt + (g % kGroupsPerWindow) * 32);
+    row[0] = make_uint4(c[0], c[1], c[2], c[3]);
+    row[1] = make_uint4(c[4], c[5], c[6], c[7]);
+  }
+}
+
+// Claims query slices of window w's emit until none is left and writes each slice's hits in record order (the window is
+// ready).  Every lane keeps the address of the next entry of each query of the slice (the same in all lanes: no shuffles);
+// corpus-local record indices are 32-bit.  Queries q0 + j >= nq have no bit in any mask, so nothing is stored for them.
+__device__ __forceinline__ void emit_claimed(const uint32_t* __restrict__ hits, uint8_t* __restrict__ win, uint32_t* __restrict__ lists,
+                                             unsigned long long stride, unsigned long long n_records, uint32_t nq,
+                                             unsigned long long w, int lane) {
   uint8_t* wr = win + w * kWinBytes;
   unsigned int* claim = reinterpret_cast<unsigned int*>(wr + kWinCtl) + 1;
-  const unsigned long long excl = __ldcg(reinterpret_cast<const unsigned long long*>(wr + kWinExcl) + lane);
+  const unsigned long long* excl = reinterpret_cast<const unsigned long long*>(wr + kWinExcl);
+  const unsigned long long r0 = w * kWindow;
+  const uint32_t cnt = (uint32_t)((n_records - r0) < kWindow ? (n_records - r0) : kWindow);   // the last window may be short
+  const uint32_t* src = hits + r0;
   for (;;) {
     uint32_t b = 0;
     if (lane == 0) b = atomicAdd(claim, 1u);
     b = __shfl_sync(0xffffffffu, b, 0);
-    if (b >= kEmitBlocks) break;
-    const unsigned long long r0 = w * kWindow + b * kEmitBlockRecs;
-    if (r0 >= n_records) continue;                   // the last window may be short
-    const uint32_t cnt = (uint32_t)((n_records - r0) < kEmitBlockRecs ? (n_records - r0) : kEmitBlockRecs);
-    const uint32_t* src = hits + r0;
-    // lane q: rank of the next hit of query q (records are 32-bit indices, so a rank fits: one shuffle per query and row of 32)
-    uint32_t pos = (uint32_t)(excl + __ldcg(reinterpret_cast<const unsigned int*>(wr + kWinBoff) + b * 32 + lane));
-    uint32_t nxt = (uint32_t)lane < cnt ? __ldcg(src + lane) : 0u;
-    for (uint32_t i = 0; i < cnt; i += 32) {
-      const uint32_t m = nxt;
-      nxt = i + 32 + lane < cnt ? __ldcg(src + i + 32 + lane) : 0u;
-      const unsigned long long rec = list_base + r0 + i + lane;
-      const uint32_t at = pos;                       // every query reads its rank from the row's start: no chain between queries
-      uint32_t add = 0;
-#pragma unroll 8
-      for (uint32_t q = 0; q < nq; ++q) {
-        const uint32_t n = emit_hits32(m, q, __shfl_sync(0xffffffffu, at, q), rec, stride, lists, lane);
-        if (lane == (int)q) add = n;
+    const uint32_t q0 = b * kEmitQueries;
+    if (q0 >= nq) break;
+    uint32_t* at[kEmitQueries];                                          // where the next hit of query q0 + j goes
+#pragma unroll
+    for (uint32_t j = 0; j < kEmitQueries; ++j) at[j] = lists + (q0 + j) * stride + __ldcg(excl + q0 + j);
+    for (uint32_t i = 0; i < cnt; i += kEmitRows * 32) {
+      uint32_t m[kEmitRows];                                              // kEmitRows rows of masks in flight at once
+#pragma unroll
+      for (uint32_t r = 0; r < kEmitRows; ++r) m[r] = i + r * 32 + lane < cnt ? __ldcg(src + i + r * 32 + lane) : 0u;   // L2: other SMs wrote them
+#pragma unroll
+      for (uint32_t r = 0; r < kEmitRows; ++r) {
+        const uint32_t rec = (uint32_t)r0 + i + r * 32 + lane;
+#pragma unroll
+        for (uint32_t j = 0; j < kEmitQueries; ++j) at[j] += emit_hits32((m[r] >> (q0 + j)) & 1u, at[j], rec, lane);
       }
-      pos = at + add;
     }
   }
 }
 
 // Window w's part of the ordered per-query lists, started by the warp that completed the window (out of line, like
 // publish_window: the row loop of k_body keeps its register allocation).  Lane q owns query q:
-//   1. count the window's hits block by block (masks of records >= n_records are not read), keep the per-block offsets, and
-//      publish the count as the window's aggregate;
+//   1. add up the window's hits from the count rows of its 128 groups (store_group_counts; no mask is read) and publish the
+//      sum as the window's aggregate;
 //   2. decoupled look-back: add up the aggregates of windows w-1, w-2, ... until one carries an inclusive prefix (or window 0
-//      is reached), then publish this window's inclusive prefix, its offsets and `ready`; the last window writes totals[q];
-//   3. emit blocks of the window until every block is claimed (emit_claimed).
+//      is reached), then publish this window's inclusive prefix, its exclusive one and `ready`; the last window writes totals[q];
+//   3. emit query slices of the window until every slice is claimed (emit_claimed).
 // Progress: a completer publishes its aggregate before it looks back, and it holds no unfinished group (its own group was
 // done when it got here, and it claims the next one only after returning).  Groups are handed out in increasing order and
 // only to resident warps, so every window it waits for is either complete -- its completer publishes the aggregate without
 // waiting for anything -- or has groups that warps still scanning will finish.
 // The time limit only guards against a scan that died: it sets err (reported by finish_timing), and the
 // window publishes its prefix anyway so that later windows do not wait on it too.
-__device__ __noinline__ void build_window_lists(const uint32_t* __restrict__ hits, uint8_t* __restrict__ win, uint64_t* __restrict__ lists,
-                                                unsigned long long stride, unsigned long long list_base, unsigned long long* __restrict__ totals,
+__device__ __noinline__ void build_window_lists(const uint32_t* __restrict__ hits, uint8_t* __restrict__ win, uint32_t* __restrict__ lists,
+                                                unsigned long long stride, unsigned long long* __restrict__ totals,
                                                 unsigned long long* __restrict__ err, unsigned long long n_records, uint32_t nq,
                                                 unsigned long long w, int lane) {
-  __threadfence();                                   // acquire side of the window counter: the other groups' masks are visible now
+  __threadfence();                                   // acquire side of the window counter: the other groups' masks and counts are visible now
   const unsigned long long r0 = w * kWindow;
   const uint32_t cnt = (uint32_t)((n_records - r0) < kWindow ? (n_records - r0) : kWindow);
-  const uint32_t* src = hits + r0;
   const bool own = lane < (int)nq;
   uint8_t* wr = win + w * kWinBytes;
-  unsigned int* boff = reinterpret_cast<unsigned int*>(wr + kWinBoff);
-  uint32_t agg = 0;
-  uint32_t nxt = (uint32_t)lane < cnt ? __ldcg(src + lane) : 0u;          // L2: other SMs wrote them
-  for (uint32_t i = 0; i < cnt; i += 32) {
-    if ((i & (kEmitBlockRecs - 1)) == 0) boff[(i / kEmitBlockRecs) * 32 + lane] = agg;
-    const uint32_t m = nxt;
-    nxt = i + 32 + lane < cnt ? __ldcg(src + i + 32 + lane) : 0u;
-    agg += count_hits32(m, nq, lane);
+  // lane l adds word l & 7 of the rows l >> 3, (l >> 3) + 4, ... (one warp load covers four whole rows): bytes 0 and 2 in lo,
+  // 1 and 3 in hi, in 16-bit halves (a window has at most 4096 hits of a query); then the four lanes of each word add theirs
+  const uint32_t* rows = reinterpret_cast<const uint32_t*>(wr + kWinCnt);
+  uint32_t lo = 0, hi = 0;
+#pragma unroll 8
+  for (uint32_t r = (uint32_t)lane >> 3; r < kGroupsPerWindow; r += 4) {
+    const uint32_t v = __ldcg(rows + r * 8 + (lane & 7));                // L2: other SMs wrote them
+    lo += v & 0x00FF00FFu; hi += (v >> 8) & 0x00FF00FFu;
   }
+  lo += __shfl_xor_sync(0xffffffffu, lo, 8); hi += __shfl_xor_sync(0xffffffffu, hi, 8);
+  lo += __shfl_xor_sync(0xffffffffu, lo, 16); hi += __shfl_xor_sync(0xffffffffu, hi, 16);
+  const uint32_t j = (uint32_t)lane >> 3;                                  // lane q holds word q & 7, whose byte q >> 3 counts query q
+  const uint32_t agg = ((j & 1u) ? hi : lo) >> (16u * (j >> 1)) & 0xFFFFu;
   unsigned long long* mine = reinterpret_cast<unsigned long long*>(wr + kWinDesc) + lane;
   unsigned long long excl = 0;
   if (w == 0) {
@@ -755,35 +774,38 @@ __device__ __noinline__ void build_window_lists(const uint32_t* __restrict__ hit
   __threadfence();
   __syncwarp();
   if (lane == 0) st_release_u32(reinterpret_cast<unsigned int*>(wr + kWinCtl), 1u);    // offsets published: anyone may emit
-  emit_claimed(hits, win, lists, stride, list_base, n_records, nq, w, lane);
+  emit_claimed(hits, win, lists, stride, n_records, nq, w, lane);
 }
 
 // A warp that finds no group left to scan helps emit the last windows of the scan [0, n_windows): the groups of those
 // windows are all handed out, so each becomes ready once its completer has looked back (see build_window_lists); a helper
-// holds no group and waits for nothing else.  Windows whose blocks are all claimed are skipped.
-__device__ __noinline__ void help_tail(const uint32_t* __restrict__ hits, uint8_t* __restrict__ win, uint64_t* __restrict__ lists,
-                                       unsigned long long stride, unsigned long long list_base, unsigned long long* __restrict__ err,
+// holds no group and waits for nothing else.  Windows whose slices are all claimed are skipped.
+__device__ __noinline__ void help_tail(const uint32_t* __restrict__ hits, uint8_t* __restrict__ win, uint32_t* __restrict__ lists,
+                                       unsigned long long stride, unsigned long long* __restrict__ err,
                                        unsigned long long n_records, uint32_t nq, unsigned long long n_windows, int lane) {
   const unsigned long long w0 = n_windows > kHelpWindows ? n_windows - kHelpWindows : 0;
+  const uint32_t slices = (nq + kEmitQueries - 1) / kEmitQueries;
   for (unsigned long long w = w0; w < n_windows; ++w) {
     const unsigned int* ctl = reinterpret_cast<const unsigned int*>(win + w * kWinBytes + kWinCtl);
-    if (__ldcg(ctl + 1) >= kEmitBlocks) continue;                // every block already taken
+    if (__ldcg(ctl + 1) >= slices) continue;                     // every slice already taken
     const long long t0 = clock64();
     while (__any_sync(0xffffffffu, ld_acquire_u32(ctl) == 0u)) {
       if (clock64() - t0 > 20000000000ll) { if (lane == 0) atomicExch(err, 1ull); return; }    // ~10 s
       __nanosleep(512);
     }
-    emit_claimed(hits, win, lists, stride, list_base, n_records, nq, w, lane);
+    emit_claimed(hits, win, lists, stride, n_records, nq, w, lane);
   }
 }
 
 // kPush: the multi-GPU instantiation; the single-GPU kernels do not carry the exchange code (it cost 0.5 % of the headline
 // when it was compiled into the one kernel: a shuffle and a branch per group, and a different register allocation).
-// kLists: k_body, which builds the ordered hit lists window by window when a.lists is set.
+// kLists: k_body, which builds the ordered hit lists window by window when a.lists is set; m is the lane's hit mask
+// (0 without a record), whose per-query counts go to the window's state before the group counts as done.
 template <bool kPush, bool kLists>
-__device__ __forceinline__ void signal_group_done(const BodyArgs& a, unsigned long long g, int lane) {
+__device__ __forceinline__ void signal_group_done(const BodyArgs& a, unsigned long long g, uint32_t m, int lane) {
   if (!a.win_done) return;
-  __threadfence();                                   // this lane's hit mask is visible device-wide ...
+  if (kLists && a.lists) store_group_counts(a.win_state, g, m, lane);
+  __threadfence();                                   // this lane's hit mask (and lane 0's count row) is visible device-wide ...
   __syncwarp();
   unsigned int old = 0;
   if (lane == 0) old = atomicAdd(a.win_done + g / kGroupsPerWindow, 1u);   // ... before the group counts as done
@@ -792,7 +814,7 @@ __device__ __forceinline__ void signal_group_done(const BodyArgs& a, unsigned lo
     if (old + 1u == kGroupsPerWindow) {
       const unsigned long long w = g / kGroupsPerWindow;
       if (kPush && a.push_n) publish_window(a.hits, a.push_peers, a.push_n, a.push_off, a.n_records, w, lane);
-      if (kLists && a.lists) build_window_lists(a.hits, a.win_state, a.lists, a.list_stride, a.list_base, a.totals, a.counter + 5, a.n_records, a.nq, w, lane);
+      if (kLists && a.lists) build_window_lists(a.hits, a.win_state, a.lists, a.list_stride, a.totals, a.counter + 5, a.n_records, a.nq, w, lane);
     }
   }
 }
@@ -964,7 +986,7 @@ __global__ void __launch_bounds__(kBodyThreads, 1) k_body(BodyArgs a) {
     const bool live = alive != 0;
     if (__ballot_sync(0xffffffffu, live) == 0) {              // nobody in this group can still match: skip its bytes
       if (rec != kInvalidRec && !a.has_alive) a.hits[rec] = 0;
-      signal_group_done<kPush, true>(a, g, lane);
+      signal_group_done<kPush, true>(a, g, 0u, lane);
       continue;
     }
     const uint8_t* row = a.tiles + a.grp_base[g] * 16;
@@ -1034,15 +1056,17 @@ __global__ void __launch_bounds__(kBodyThreads, 1) k_body(BodyArgs a) {
       if (kAcc != 3 && k1 < lim && dec.decided(d)) lim = k1;
       if (__ballot_sync(0xffffffffu, k1 < lim) == 0) break;
     }
+    uint32_t hit = 0;
     if (live) {
-      a.hits[rec] = content_hits(d.finish(endout), alive, queries, conds, nq);
+      hit = content_hits(d.finish(endout), alive, queries, conds, nq);
+      a.hits[rec] = hit;
     } else if (rec != kInvalidRec && !a.has_alive) {
       a.hits[rec] = 0;
     }
-    signal_group_done<kPush, true>(a, g, lane);
+    signal_group_done<kPush, true>(a, g, hit, lane);
   }
   if (a.lists && a.win_done)                       // no group left: help write the lists of the scan's last windows
-    help_tail(a.hits, a.win_state, a.lists, a.list_stride, a.list_base, a.counter + 5, a.n_records, a.nq,
+    help_tail(a.hits, a.win_state, a.lists, a.list_stride, a.counter + 5, a.n_records, a.nq,
               a.n_groups / kGroupsPerWindow, lane);
   unsigned long long bytes_read = 16ull * rows_read;
   for (int o = 16; o; o >>= 1) bytes_read += __shfl_down_sync(0xffffffffu, bytes_read, o);
@@ -1312,8 +1336,8 @@ __global__ void __launch_bounds__(kBodyThreads, 1) k_body_sticky(BodyArgs a) {
     ragged_pair(A, B);
     close_group(A);
     close_group(B);
-    signal_group_done<kPush, false>(a, g, lane);
-    if (g + 1 < a.n_groups) signal_group_done<kPush, false>(a, g + 1, lane);
+    signal_group_done<kPush, false>(a, g, 0u, lane);
+    if (g + 1 < a.n_groups) signal_group_done<kPush, false>(a, g + 1, 0u, lane);
   }
   if (lane == 0 && touched) { atomicAdd(a.counter + 1, touched); atomicAdd(a.counter + 3, bytes_read); }
 }
@@ -1461,19 +1485,21 @@ __global__ void k_scan_blocks(const uint32_t* __restrict__ counts, uint64_t nblo
   if (threadIdx.x == 0) carry_io[q] = carry;
 }
 
-// ordered emit: lists[q * stride + rank] = global_base + i
+// ordered emit: lists[q * stride + rank] = base + i -- corpus-local 32-bit indices (base 0) for a corpus' own lists, 64-bit
+// global ones for the lists built from gathered rank segments (comm.cu)
 // (a resident scan CTA of k_body holds the whole register file, so these kernels run between scans, not under one)
+template <class T>
 __global__ void __launch_bounds__(kCompactBlock, 8)
 k_emit(const uint32_t* __restrict__ hits, uint64_t n, uint32_t nq, const uint64_t* __restrict__ offsets,
-       uint64_t global_base, uint64_t stride, uint64_t* __restrict__ lists) {
+       T base, uint64_t stride, T* __restrict__ lists) {
   __shared__ uint32_t wcnt[8][32];          // [warp][query] hits of this warp's records
   const uint64_t blk = blockIdx.x;
-  uint64_t base = blk * kCompactRecs;
+  const uint64_t first = blk * kCompactRecs;
   int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   uint32_t m[kCompactPer];
   uint32_t cnt = 0;
   for (int r = 0; r < kCompactPer; ++r) {
-    uint64_t i = base + (uint64_t)(warp * kCompactPer + r) * 32 + lane;
+    uint64_t i = first + (uint64_t)(warp * kCompactPer + r) * 32 + lane;
     m[r] = i < n ? hits[i] : 0u;
     cnt += count_hits32(m[r], nq, lane);
   }
@@ -1482,19 +1508,26 @@ k_emit(const uint32_t* __restrict__ hits, uint64_t n, uint32_t nq, const uint64_
   for (uint32_t q = 0; q < nq; ++q) {
     uint64_t pos = offsets[blk * nq + q];
     for (int w = 0; w < warp; ++w) pos += wcnt[w][q];
+    T* list = lists + q * stride;
     for (int r = 0; r < kCompactPer; ++r)
-      pos += emit_hits32(m[r], q, pos, global_base + base + (uint64_t)(warp * kCompactPer + r) * 32 + lane, stride, lists, lane);
+      pos += emit_hits32<T>((m[r] >> q) & 1u, list + pos, base + (T)(first + (uint64_t)(warp * kCompactPer + r) * 32 + lane), lane);
   }
 }
 
-// Ordered lists of the n masks at `masks` (record 0 is global index global_base) into lists[q * stride + rank], the ranks
-// continuing from sc.totals, which is left holding the running per-query totals.  n > 0.
-static void compact_lists(const uint32_t* masks, uint64_t n, uint32_t nq, uint64_t global_base, CompactScratch& sc, uint64_t stride,
-                          uint64_t* lists, cudaStream_t s) {
+// Ordered lists of the n masks at `masks` (record 0 is index `base`) into lists[q * stride + rank], the ranks continuing
+// from sc.totals, which is left holding the running per-query totals.  n > 0.
+template <class T>
+static void compact_lists(const uint32_t* masks, uint64_t n, uint32_t nq, T base, CompactScratch& sc, uint64_t stride,
+                          T* lists, cudaStream_t s) {
   const uint64_t nb = (n + kCompactRecs - 1) / kCompactRecs;
   k_count<<<(unsigned)nb, kCompactBlock, 0, s>>>(masks, n, nq, sc.blk_counts.as<uint32_t>());
   k_scan_blocks<<<nq, 256, 0, s>>>(sc.blk_counts.as<uint32_t>(), nb, nq, sc.blk_offsets.as<uint64_t>(), sc.totals.as<uint64_t>());
-  k_emit<<<(unsigned)nb, kCompactBlock, 0, s>>>(masks, n, nq, sc.blk_offsets.as<uint64_t>(), global_base, stride, lists);
+  k_emit<T><<<(unsigned)nb, kCompactBlock, 0, s>>>(masks, n, nq, sc.blk_offsets.as<uint64_t>(), base, stride, lists);
+}
+
+// dst[i] = base + src[i]: corpus-local list entries as global indices
+__global__ void k_widen(const uint32_t* __restrict__ src, uint64_t n, uint64_t base, uint64_t* __restrict__ dst) {
+  for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) dst[i] = base + src[i];
 }
 
 __global__ void k_fill32(uint32_t* __restrict__ p, uint64_t n, uint32_t v) {
@@ -1502,12 +1535,16 @@ __global__ void k_fill32(uint32_t* __restrict__ p, uint64_t n, uint32_t v) {
   if (i < n) p[i] = v;
 }
 
-// Order-sensitive checksum of an index list: sum_k (k + 1) * v[k] and sum_k v[k] (mod 2^64).  Two lists agree on both
-// sums iff (with overwhelming probability) they hold the same indices in the same order; the pair (A, S) of the
-// concatenation of two lists follows from the parts: A = A1 + A2 + len1 * S2.
-__global__ void __launch_bounds__(256) k_list_checksum(const uint64_t* __restrict__ v, uint64_t n, unsigned long long* __restrict__ out) {
+// Order-sensitive checksum of an index list (entry k is index base + v[k]): sum_k (k + 1) * index_k and sum_k index_k
+// (mod 2^64).  Two lists agree on both sums iff (with overwhelming probability) they hold the same indices in the same order;
+// the pair (A, S) of the concatenation of two lists follows from the parts: A = A1 + A2 + len1 * S2.
+template <class T>
+__global__ void __launch_bounds__(256) k_list_checksum(const T* __restrict__ v, uint64_t n, unsigned long long base, unsigned long long* __restrict__ out) {
   unsigned long long a = 0, s = 0;
-  for (uint64_t k = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; k < n; k += (uint64_t)gridDim.x * blockDim.x) { a += (k + 1) * v[k]; s += v[k]; }
+  for (uint64_t k = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; k < n; k += (uint64_t)gridDim.x * blockDim.x) {
+    const unsigned long long x = base + v[k];
+    a += (k + 1) * x; s += x;
+  }
   for (int o = 16; o; o >>= 1) { a += __shfl_down_sync(0xffffffffu, a, o); s += __shfl_down_sync(0xffffffffu, s, o); }
   if ((threadIdx.x & 31) == 0) { atomicAdd(out, a); atomicAdd(out + 1, s); }
 }
@@ -1577,7 +1614,7 @@ int run_scan(fei_corpus* c, const uint8_t* prog, uint64_t prog_len, int compact_
     FEI_TRY(c->compact.blk_counts.ensure((nblocks ? nblocks : 1) * nq * sizeof(uint32_t)));
     FEI_TRY(c->compact.blk_offsets.ensure((nblocks ? nblocks : 1) * nq * sizeof(uint64_t)));
     FEI_TRY(c->compact.totals.ensure(32 * sizeof(uint64_t)));
-    FEI_TRY(c->hit_lists.ensure((n ? n : 1) * nq * sizeof(uint64_t)));
+    FEI_TRY(c->hit_lists.ensure((n ? n : 1) * nq * sizeof(uint32_t)));
     c->hit_list_stride = n ? n : 1;
     FEI_CUDA(cudaMemsetAsync(c->compact.totals.p, 0, 32 * sizeof(uint64_t), s));
   }
@@ -1690,7 +1727,7 @@ int run_scan(fei_corpus* c, const uint8_t* prog, uint64_t prog_len, int compact_
     FEI_TRY(c->win_state.ensure(n_windows * kWinBytes));
     FEI_CUDA(cudaMemsetAsync(c->win_state.p, 0, n_windows * kWinBytes, s));
     a.win_state = c->win_state.as<uint8_t>();
-    a.lists = c->hit_lists.as<uint64_t>(); a.list_stride = c->hit_list_stride; a.list_base = c->global_base;
+    a.lists = c->hit_lists.as<uint32_t>(); a.list_stride = c->hit_list_stride;
     a.totals = c->compact.totals.as<unsigned long long>(); a.nq = nq;
   }
   if (push) { a.push_peers = hook->push_peers; a.push_n = hook->push_n; a.push_off = hook->push_off; hook->pushed = true; }
@@ -1701,7 +1738,7 @@ int run_scan(fei_corpus* c, const uint8_t* prog, uint64_t prog_len, int compact_
   }
   FEI_CUDA(cudaEventRecord(c->ev[3], s));
   if (n && compact_mode == kCompactLists && !body_lists) {
-    compact_lists(c->hits.as<uint32_t>(), n, nq, c->global_base, c->compact, c->hit_list_stride, c->hit_lists.as<uint64_t>(), s);
+    compact_lists<uint32_t>(c->hits.as<uint32_t>(), n, nq, 0u, c->compact, c->hit_list_stride, c->hit_lists.as<uint32_t>(), s);
     launches += 3;
   }
   if (hook) FEI_TRY(hook->after_scan(s));
@@ -1756,7 +1793,8 @@ int compact_masks(const uint32_t* masks, uint64_t n, uint32_t nq, uint64_t globa
     for (uint32_t q = 0; q < nq; ++q) if (counts_out[q] > stride) stride = counts_out[q];
     if (stride_out) *stride_out = stride;
     FEI_TRY(lists->ensure(stride * nq * sizeof(uint64_t)));
-    k_emit<<<(unsigned)nblocks, kCompactBlock, 0, s>>>(masks, n, nq, sc.blk_offsets.as<uint64_t>(), global_base, stride, lists->as<uint64_t>());
+    k_emit<unsigned long long><<<(unsigned)nblocks, kCompactBlock, 0, s>>>(masks, n, nq, sc.blk_offsets.as<uint64_t>(), global_base, stride,
+                                                                         lists->as<unsigned long long>());
     if (launches) *launches += 1;
   }
   FEI_CUDA(cudaGetLastError());
@@ -1775,7 +1813,8 @@ int compact_segments(const uint32_t* masks, uint64_t seg_stride, const uint64_t*
   FEI_TRY(sc.totals.ensure(32 * sizeof(uint64_t)));
   FEI_CUDA(cudaMemsetAsync(sc.totals.p, 0, 32 * sizeof(uint64_t), s));
   for (uint32_t r = 0; r < n_seg; ++r)                         // the totals run on across segments
-    if (seg_n[r]) compact_lists(masks + (size_t)r * seg_stride, seg_n[r], nq, seg_base[r], sc, stride, lists, s);
+    if (seg_n[r]) compact_lists<unsigned long long>(masks + (size_t)r * seg_stride, seg_n[r], nq, seg_base[r], sc, stride,
+                                                    reinterpret_cast<unsigned long long*>(lists), s);
   if (totals_out) {
     FEI_CUDA(cudaMemcpyAsync(totals_out, sc.totals.p, nq * sizeof(uint64_t), cudaMemcpyDeviceToHost, s));
     FEI_CUDA(cudaStreamSynchronize(s));
@@ -1784,15 +1823,48 @@ int compact_segments(const uint32_t* masks, uint64_t seg_stride, const uint64_t*
   return FEI_OK;
 }
 
-// (A, S) checksums of `count` indices at `list` (device memory); see k_list_checksum
-int list_checksum(const uint64_t* list, uint64_t count, DevBuf& tmp, uint64_t* a_out, uint64_t* s_out, cudaStream_t s) {
+// (A, S) checksums of `count` indices base + list[k] (device memory); see k_list_checksum
+template <class T>
+static int list_checksum_of(const T* list, uint64_t count, uint64_t base, DevBuf& tmp, uint64_t* a_out, uint64_t* s_out, cudaStream_t s) {
   FEI_TRY(tmp.ensure(16));
   FEI_CUDA(cudaMemsetAsync(tmp.p, 0, 16, s));
-  if (count) k_list_checksum<<<(unsigned)std::min<uint64_t>((count + 255) / 256, 4096), 256, 0, s>>>(list, count, tmp.as<unsigned long long>());
+  if (count) k_list_checksum<T><<<(unsigned)std::min<uint64_t>((count + 255) / 256, 4096), 256, 0, s>>>(list, count, base, tmp.as<unsigned long long>());
   unsigned long long r[2];
   FEI_CUDA(cudaMemcpyAsync(r, tmp.p, 16, cudaMemcpyDeviceToHost, s));
   FEI_CUDA(cudaStreamSynchronize(s));
   *a_out = r[0]; *s_out = r[1];
+  return FEI_OK;
+}
+int list_checksum(const uint64_t* list, uint64_t count, DevBuf& tmp, uint64_t* a_out, uint64_t* s_out, cudaStream_t s) {
+  return list_checksum_of(list, count, 0, tmp, a_out, s_out, s);
+}
+int list_checksum(const uint32_t* list, uint64_t count, uint64_t base, DevBuf& tmp, uint64_t* a_out, uint64_t* s_out, cudaStream_t s) {
+  return list_checksum_of(list, count, base, tmp, a_out, s_out, s);
+}
+
+int widen_list(const uint32_t* src, uint64_t n, uint64_t base, uint64_t* dst, cudaStream_t s) {
+  if (n) k_widen<<<(unsigned)std::min<uint64_t>((n + 255) / 256, 4096), 256, 0, s>>>(src, n, base, dst);
+  FEI_CUDA(cudaGetLastError());
+  return FEI_OK;
+}
+
+// Copies (a prefix of) every query's list of the last scan to the host as global indices: each list is widened on the device
+// into c->list_stage (one buffer, reused in stream order) and copied from there.  *truncated: some cap[q] was too small.
+static int copy_lists_out(fei_corpus* c, uint32_t nq, uint64_t* const* hits, const uint64_t* cap, bool* truncated, cudaStream_t s) {
+  uint64_t most = 0;
+  for (uint32_t q = 0; q < nq; ++q) {
+    const uint64_t take = c->last_counts[q] < cap[q] ? c->last_counts[q] : cap[q];
+    if (take < c->last_counts[q]) *truncated = true;
+    if (hits[q] && take > most) most = take;
+  }
+  if (!most) return FEI_OK;
+  FEI_TRY(c->list_stage.ensure(most * sizeof(uint64_t)));
+  for (uint32_t q = 0; q < nq; ++q) {
+    const uint64_t take = c->last_counts[q] < cap[q] ? c->last_counts[q] : cap[q];
+    if (!take || !hits[q]) continue;
+    FEI_TRY(widen_list(c->hit_lists.as<uint32_t>() + q * c->hit_list_stride, take, c->global_base, c->list_stage.as<uint64_t>(), s));
+    FEI_CUDA(cudaMemcpyAsync(hits[q], c->list_stage.p, take * sizeof(uint64_t), cudaMemcpyDeviceToHost, s));
+  }
   return FEI_OK;
 }
 
@@ -1826,12 +1898,8 @@ extern "C" int fei_scan_hits(fei_corpus* c, const uint8_t* prog, uint64_t prog_l
   cudaStream_t s = ctx().stream;
   FEI_CUDA(cudaStreamSynchronize(s));                                  // the counts decide how much of every list is copied
   bool truncated = false;
-  for (uint32_t q = 0; q < c->last_nq; ++q) {
-    nhits[q] = c->last_counts[q];
-    uint64_t take = nhits[q] < cap[q] ? nhits[q] : cap[q];
-    if (take < nhits[q]) truncated = true;
-    if (take && hits[q]) FEI_CUDA(cudaMemcpyAsync(hits[q], c->hit_lists.as<uint64_t>() + q * c->hit_list_stride, take * 8, cudaMemcpyDeviceToHost, s));
-  }
+  for (uint32_t q = 0; q < c->last_nq; ++q) nhits[q] = c->last_counts[q];
+  FEI_TRY(copy_lists_out(c, c->last_nq, hits, cap, &truncated, s));
   FEI_TRY(finish_timing(c, true));
   if (truncated) { set_error("hit buffer too small for at least one query (see nhits)"); return FEI_E_CAPACITY; }
   return FEI_OK;
@@ -1844,11 +1912,7 @@ extern "C" int fei_scan_fetch_hits(fei_corpus* c, uint32_t nq, uint64_t* const* 
   if (nq == 0 || nq != c->last_nq || !c->hit_lists.p) { set_error("no matching scan result with lists on this corpus"); return FEI_E_STATE; }
   cudaStream_t s = ctx().stream;
   bool truncated = false;
-  for (uint32_t q = 0; q < nq; ++q) {
-    uint64_t take = c->last_counts[q] < cap[q] ? c->last_counts[q] : cap[q];
-    if (take < c->last_counts[q]) truncated = true;
-    if (take && hits[q]) FEI_CUDA(cudaMemcpyAsync(hits[q], c->hit_lists.as<uint64_t>() + q * c->hit_list_stride, take * 8, cudaMemcpyDeviceToHost, s));
-  }
+  FEI_TRY(copy_lists_out(c, nq, hits, cap, &truncated, s));
   FEI_CUDA(cudaStreamSynchronize(s));
   if (truncated) { set_error("hit buffer too small for at least one query"); return FEI_E_CAPACITY; }
   return FEI_OK;
@@ -1860,7 +1924,7 @@ extern "C" int fei_scan_list_checksum(fei_corpus* c, uint32_t nq, uint64_t* a_ou
   std::lock_guard<std::mutex> lock(c->mu);
   if (nq == 0 || nq != c->last_nq || !c->hit_lists.p) { set_error("no matching scan result with lists on this corpus"); return FEI_E_STATE; }
   for (uint32_t q = 0; q < nq; ++q)
-    FEI_TRY(list_checksum(c->hit_lists.as<uint64_t>() + q * c->hit_list_stride, c->last_counts[q], c->scan_tmp, a_out + q, s_out + q, ctx().stream));
+    FEI_TRY(list_checksum(c->hit_lists.as<uint32_t>() + q * c->hit_list_stride, c->last_counts[q], c->global_base, c->scan_tmp, a_out + q, s_out + q, ctx().stream));
   return FEI_OK;
 }
 

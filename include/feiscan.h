@@ -205,10 +205,14 @@ int fei_scan_masks(fei_corpus* c, const uint8_t* prog, uint64_t prog_len, uint32
 int fei_scan_hits(fei_corpus* c, const uint8_t* prog, uint64_t prog_len,
                   uint64_t* const* hits, const uint64_t* cap, uint64_t* nhits);
 /* Counts on the host, the ordered lists stay on the device: nhits[q] for every query.
- * The multi-pattern body kernel builds the lists itself while it scans: the warp that
- * completes a 4096-record window writes that window's part of every list (warps that have
- * nothing left to scan help with the last windows).  Single-pattern
- * content scans and header-only programs compact the finished masks with separate kernels. */
+ * The multi-pattern body kernel builds the lists itself while it scans: every warp leaves
+ * the per-query counts of the 32 records it finished, and the warp that completes a
+ * 4096-record window adds them up and writes that window's part of every list (warps that
+ * have nothing left to scan help with the last windows).  Single-pattern content scans and
+ * header-only programs compact the finished masks with separate kernels.  On the device a
+ * list entry is a 4-byte record index local to the corpus; the calls below that hand lists
+ * out (fei_scan_hits, fei_scan_fetch_hits, fei_scan_list_checksum) add global_base on the
+ * device and give 64-bit global indices.                                                   */
 int fei_scan_count(fei_corpus* c, const uint8_t* prog, uint64_t prog_len, uint64_t* nhits);
 /* Copies the lists the last fei_scan_count left on the device (hits[q] has room for cap[q]
  * entries; FEI_E_CAPACITY if one is shorter than its list): the second half of fei_scan_hits

@@ -6,7 +6,8 @@
 A round is one process per library (A, then B): it builds the synthetic bench corpus (two corpora of 10 M entries do not
 fit one 80 GB card, so the libraries take turns) and runs `--calls` scan_count calls of the 32-pattern bench batch and of
 a batch of 32 words that occur nowhere (every byte goes through the automaton, no record is ever decided), printing the
-median body_ms / total_ms of each from Corpus.timing().  The card's name, power limit and SM clock are printed last: they
+median body_ms / total_ms of each from Corpus.timing().  Every scan_count call is followed by a scan_masks call of the same
+batch (the same kernel without the ordered lists): the difference of their body_ms medians is what building the lists costs.  The card's name, power limit and SM clock are printed last: they
 belong to every number above.  Exits non-zero without a GPU."""
 import argparse, json, os, re, statistics, subprocess, sys
 
@@ -36,12 +37,16 @@ def worker(lib_path, entries, calls):
         prog = content_batch_program([Pattern("regex", p, re.IGNORECASE) for p in pats])
         for _ in range(3):
             cnt = c.scan_count(prog, 32)
-        body, total = [], []
+            c.scan_masks(prog)
+        body, total, masks_body = [], [], []
         for _ in range(calls):
             cnt = c.scan_count(prog, 32)
             tm = c.timing()
             body.append(tm["body_ms"]); total.append(tm["total_ms"])
+            c.scan_masks(prog)
+            masks_body.append(c.timing()["body_ms"])
         out[name] = {"body_ms": statistics.median(body), "total_ms": statistics.median(total), "hits": int(cnt.sum()),
+                     "masks_body_ms": statistics.median(masks_body),
                      "body_bytes_read": int(tm["body_bytes_read"]),
                      "kernel": [int(tm["body_kernel"]), int(tm["body_direct"]), int(tm["body_acc_mode"])]}
     print(json.dumps(out))
@@ -74,14 +79,18 @@ def main():
             out = json.loads(p.stdout.strip().splitlines()[-1])
             for name, o in out.items():
                 res[lib][name].append(o)
-                print(f"round {r} {lib:40s} {name:9s} body_ms {o['body_ms']:7.3f}  total_ms {o['total_ms']:7.3f}  hits {o['hits']}  "
+                print(f"round {r} {lib:40s} {name:9s} body_ms {o['body_ms']:7.3f}  masks-only body_ms {o['masks_body_ms']:7.3f}  "
+                      f"total_ms {o['total_ms']:7.3f}  hits {o['hits']}  "
                       f"body_bytes_read {o['body_bytes_read']}  kernel/direct/acc {o['kernel']}", flush=True)
     print()
     for name in ("batch32", "absent32"):
         for lib in args.libs:
             b = [o["body_ms"] for o in res[lib][name]]; t = [o["total_ms"] for o in res[lib][name]]
+            mb = [o["masks_body_ms"] for o in res[lib][name]]; share = [o["body_ms"] - o["masks_body_ms"] for o in res[lib][name]]
             print(f"{name:9s} {lib:40s} body_ms median {statistics.median(b):7.3f} (range {min(b):.3f}-{max(b):.3f})  "
-                  f"total_ms median {statistics.median(t):7.3f} (range {min(t):.3f}-{max(t):.3f})")
+                  f"total_ms median {statistics.median(t):7.3f} (range {min(t):.3f}-{max(t):.3f})  "
+                  f"masks-only body_ms median {statistics.median(mb):7.3f}  lists share median {statistics.median(share):6.3f} "
+                  f"(range {min(share):.3f}-{max(share):.3f})")
         same = len({(o["hits"], o["body_bytes_read"]) for lib in args.libs for o in res[lib][name]}) == 1
         print(f"{name:9s} hits and body_bytes_read equal in every run: {same}")
     print("GPU (name, power limit, SM clock now, SM clock max):", gpu.splitlines()[0])
