@@ -24,6 +24,8 @@
 //          and the warp that completes a window of 4096 records adds them up and appends the window's hits
 //          to the per-query ordered lists of 32-bit corpus-local indices (build_window_lists: decoupled
 //          look-back over the windows); warps with no group left help write the last windows' lists (help_tail).
+// k_body_nfa : content patterns too large for the DFA, stepped per code point as a bit-parallel position automaton (next to the
+//          DFA of the program's other content patterns); same group loop, lists compacted after it.
 // k_count / k_scan_blocks / k_emit : order-preserving compaction of hits[] into per-query lists
 //          (warp ballots + popc prefix, block offsets from a scan): corpus-local 32-bit indices for the
 //          single-pattern kernels and header-only programs, 64-bit global ones for gathered multi-GPU masks.
@@ -1410,9 +1412,233 @@ __global__ void __launch_bounds__(kBodyThreads, 1) k_body_gather(BodyArgs a, con
   if ((threadIdx.x & 31) == 0 && bytes_read) { atomicAdd(a.counter + 3, bytes_read); atomicAdd(a.counter + 1, bytes_read); }
 }
 
+// ---------------------------------------------------------------- content position automaton (bit-parallel NFA)
+// k_body_nfa: content patterns whose DFA is too large (bounded gaps: `a.{0,60}b`) run as a position automaton
+// (feiscan_prog.h fei_prog_nfa): per code point, a W-word bit vector of NFA positions steps through
+//     D' = (((D << 1) & SHIFT) | (D & SELF) | OR_g [(D & src_g) && ctx ok] dst_g) & B[class]
+// The group loop is k_body's (warps claim 32-record groups, one lane per record, 16-byte rows, groups with no live record
+// skipped); each lane undoes the tile byte permutation, decodes UTF-8 and looks the class up (ASCII table, else a binary
+// search over the range table).  A program that also has a body DFA (class-indexed, not sticky) steps it on every byte as
+// k_body<false, 0> does; its outputs are the content bits below the automaton's first_bit.  The ordered lists are compacted
+// after the scan and the multi-GPU hook copies the masks (no window work in the kernel).
+template <int W> struct NfaThreads { static constexpr int value = W <= 4 ? 1024 : 512; };
+
+struct NfaTables {                   // shared-memory views of a staged fei_prog_nfa
+  const uint16_t* ascii; const uint32_t* range_lo; const uint16_t* range_ck; const uint32_t* cls_b;
+  const uint32_t* masks; const uint32_t* follow; const uint32_t* accept;
+  uint32_t n_ranges, n_follow, n_accept;
+  __device__ __forceinline__ uint32_t class_kind(uint32_t cp) const {     // class | kind << 8
+    if (cp < 0x80u) return ascii[cp];
+    uint32_t lo = 0, hi = n_ranges - 1;
+    while (lo < hi) {
+      const uint32_t mid = (lo + hi + 1) >> 1;
+      if (range_lo[mid] <= cp) lo = mid; else hi = mid - 1;
+    }
+    return range_ck[lo];
+  }
+};
+
+template <int W>
+struct BodyNfa {
+  uint32_t d[W];                     // active positions
+  uint32_t prev;                     // context kind of the last code point (0: none yet)
+  uint32_t cp, need;                 // UTF-8 decoder: code point so far, continuation bytes still to come
+  uint32_t acc;                      // output bits of the accepts met so far (end-only accepts not included)
+  __device__ __forceinline__ void reset(const NfaTables& t) {
+#pragma unroll
+    for (int k = 0; k < W; ++k) d[k] = t.masks[2 * W + k];
+    prev = 0; cp = 0; need = 0; acc = 0;
+  }
+  __device__ __forceinline__ bool any(const uint32_t* src) const {
+    uint32_t x = 0;
+#pragma unroll
+    for (int k = 0; k < W; ++k) x |= d[k] & src[k];
+    return x != 0;
+  }
+  __device__ __forceinline__ uint32_t accepts(const NfaTables& t, uint32_t ctx, bool at_end) const {
+    uint32_t m = 0;
+    for (uint32_t g = 0; g < t.n_accept; ++g) {
+      const uint32_t* r = t.accept + g * (W + 2);
+      const uint32_t info = r[W + 1];
+      if ((r[W] & ctx) && (at_end || !(info >> 8)) && any(r)) m |= 1u << (info & 31u);
+    }
+    return m;
+  }
+  __device__ __forceinline__ void step_cp(const NfaTables& t, uint32_t c) {
+    const uint32_t ck = t.class_kind(c);
+    const uint32_t kind = ck >> 8;
+    const uint32_t ctx = 1u << (prev * 5u + kind);
+    acc |= accepts(t, ctx, false);
+    uint32_t n[W];
+#pragma unroll
+    for (int k = 0; k < W; ++k) {
+      const uint32_t sh = k ? __funnelshift_l(d[k - 1], d[k], 1) : d[0] << 1;
+      n[k] = (sh & t.masks[k]) | (d[k] & t.masks[W + k]);
+    }
+    for (uint32_t g = 0; g < t.n_follow; ++g) {
+      const uint32_t* r = t.follow + g * (2 * W + 1);
+      if ((r[2 * W] & ctx) && any(r)) {
+#pragma unroll
+        for (int k = 0; k < W; ++k) n[k] |= r[W + k];
+      }
+    }
+    const uint32_t* b = t.cls_b + (ck & 0xFFu) * W;
+#pragma unroll
+    for (int k = 0; k < W; ++k) d[k] = n[k] & b[k];
+    prev = kind;
+  }
+  // one stored tile byte
+  __device__ __forceinline__ void byte(const NfaTables& t, uint32_t stored) {
+    const uint32_t b = tile_byte_unperm((uint8_t)stored);
+    if (b < 0x80u) { step_cp(t, b); return; }                        // ASCII: one byte, one code point
+    if (b >= 0xC0u) { need = b >= 0xF0u ? 3u : b >= 0xE0u ? 2u : 1u; cp = b & (0x3Fu >> need); return; }
+    cp = (cp << 6) | (b & 0x3Fu);
+    if (--need == 0) step_cp(t, cp);
+  }
+  __device__ __forceinline__ uint32_t finish(const NfaTables& t) const { return acc | accepts(t, 1u << (prev * 5u), true); }
+};
+
+// Stage the body DFA's tables (bytes0, may be 0) and the position automaton's behind them with one mbarrier.
+__device__ __forceinline__ void stage_two_tables(uint8_t* dst0, const uint8_t* src0, uint32_t bytes0, uint8_t* dst1, const uint8_t* src1,
+                                                 uint32_t bytes1, uint64_t* bar) {
+  if (threadIdx.x == 0) { mbar_init(bar, 1); asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    mbar_expect_tx(bar, bytes0 + bytes1);
+    for (uint32_t o = 0; o < bytes0; o += 32768u) bulk_g2s(dst0 + o, src0 + o, bytes0 - o < 32768u ? bytes0 - o : 32768u, bar);
+    for (uint32_t o = 0; o < bytes1; o += 32768u) bulk_g2s(dst1 + o, src1 + o, bytes1 - o < 32768u ? bytes1 - o : 32768u, bar);
+  }
+  mbar_wait(bar, 0);
+}
+
+template <int W, bool kHasDfa>
+__global__ void __launch_bounds__(NfaThreads<W>::value, 1) k_body_nfa(BodyArgs a) {
+  extern __shared__ __align__(128) uint8_t smem[];
+  __shared__ uint64_t bar;
+  __shared__ uint32_t q_need[33];                  // as in k_body
+  const fei_prog_hdr* ph = reinterpret_cast<const fei_prog_hdr*>(a.prog);
+  const fei_prog_nfa* nd = reinterpret_cast<const fei_prog_nfa*>(a.prog + ph->off_body_nfa);
+  const fei_prog_dfa* dd = reinterpret_cast<const fei_prog_dfa*>(a.prog + ph->off_body_dfa);
+  const fei_prog_cond* conds = reinterpret_cast<const fei_prog_cond*>(a.prog + ph->off_conds);
+  const fei_prog_query* queries = reinterpret_cast<const fei_prog_query*>(a.prog + ph->off_queries);
+  const uint32_t nq = ph->n_queries;
+  if (threadIdx.x < 32) {
+    uint32_t bits = 0;
+    if (threadIdx.x < nq)
+      for (uint32_t c = queries[threadIdx.x].cond_begin; c < queries[threadIdx.x].cond_end; ++c)
+        if (conds[c].kind == FEI_C_BODY) bits |= 1u << conds[c].bit;
+    q_need[threadIdx.x] = bits;
+    bits = __reduce_or_sync(0xffffffffu, bits);
+    if (threadIdx.x == 0) q_need[32] = bits;
+  }
+  const uint32_t dfa_bytes = kHasDfa ? dd->table_bytes : 0u;
+  uint8_t* nsm = smem + dfa_bytes;                 // both table sizes are multiples of 16
+  stage_two_tables(smem, kHasDfa ? a.prog + dd->off_trans : nullptr, dfa_bytes, nsm, a.prog + nd->off_ascii, nd->table_bytes, &bar);
+  NfaTables t;
+  t.ascii = reinterpret_cast<const uint16_t*>(nsm);
+  t.range_lo = reinterpret_cast<const uint32_t*>(nsm + (nd->off_range_lo - nd->off_ascii));
+  t.range_ck = reinterpret_cast<const uint16_t*>(nsm + (nd->off_range_ck - nd->off_ascii));
+  t.cls_b = reinterpret_cast<const uint32_t*>(nsm + (nd->off_cls_b - nd->off_ascii));
+  t.masks = reinterpret_cast<const uint32_t*>(nsm + (nd->off_masks - nd->off_ascii));
+  t.follow = reinterpret_cast<const uint32_t*>(nsm + (nd->off_follow - nd->off_ascii));
+  t.accept = reinterpret_cast<const uint32_t*>(nsm + (nd->off_accept - nd->off_ascii));
+  t.n_ranges = nd->n_ranges; t.n_follow = nd->n_follow; t.n_accept = nd->n_accept;
+  BodyDfa<false, 0> d;
+  const uint32_t* endout = nullptr;
+  uint32_t dfa_start = 0;
+  if constexpr (kHasDfa) {
+    d.trans_s = smem_u32(smem);
+    d.out = reinterpret_cast<const uint32_t*>(smem + (dd->off_out - dd->off_trans));
+    d.cls = smem + (dd->off_cls - dd->off_trans);
+    d.stride2 = dd->row_stride * 2u; d.n_acc = dd->n_acc; d.entry_bytes = c_entry_bytes;
+    endout = reinterpret_cast<const uint32_t*>(smem + (dd->off_endout - dd->off_trans));
+    dfa_start = dd->start;
+  }
+  BodyNfa<W> nfa;
+  const uint32_t all_q = nq >= 32 ? 0xFFFFFFFFu : ((1u << nq) - 1u);
+  const int lane = threadIdx.x & 31;
+  unsigned long long touched = 0;
+  uint32_t rows_read = 0;
+  for (;;) {
+    unsigned long long g = 0;
+    if (lane == 0) g = atomicAdd(a.next, 1ull);
+    g = __shfl_sync(0xffffffffu, g, 0);
+    if (g >= a.n_groups) break;
+    const uint32_t rec = a.grp_rec[g * 32 + lane];
+    const uint32_t len = a.grp_len[g * 32 + lane];
+    const uint32_t units = (len + 15) >> 4;
+    uint32_t alive = 0;
+    if (rec != kInvalidRec) alive = a.has_alive ? a.hits[rec] : all_q;
+    const bool live = alive != 0;
+    if (__ballot_sync(0xffffffffu, live) == 0) {              // nobody in this group can still match: skip its bytes
+      if (rec != kInvalidRec && !a.has_alive) a.hits[rec] = 0;
+      continue;
+    }
+    const uint8_t* row = a.tiles + a.grp_base[g] * 16;
+    const uint32_t maxu = __shfl_sync(0xffffffffu, units, 0);
+    if (lane == 0) touched += (a.grp_base[g + 1] - a.grp_base[g]) * 16;
+    nfa.reset(t);
+    if constexpr (kHasDfa) d.reset(dfa_start);
+    // the content bits this lane's alive queries read; the lane stops once the accepts met so far set all of them (bits that
+    // only end-only accepts or the DFA's endout[] set keep it reading to the end)
+    uint32_t need = 0;
+    if (live) {
+      need = q_need[32];
+      if (alive != all_q) {
+        need = 0;
+        for (uint32_t q = alive; q; q &= q - 1) need |= q_need[__ffs(q) - 1];
+      }
+    }
+    auto decided = [&]() { return (need & ~(nfa.acc | (kHasDfa ? d.a0 : 0u))) == 0; };
+    uint32_t lim = live && !decided() ? units : 0;
+    uint4 cur = make_uint4(0, 0, 0, 0);
+    if (0 < lim) { cur = ldg_stream16(row + lane * 16); ++rows_read; }
+    for (uint32_t k = 0; k < maxu; ++k) {
+      const uint32_t m = __popc(__ballot_sync(0xffffffffu, k < units));
+      const uint8_t* next_row = row + (uint64_t)m * 16;
+      uint4 nxt = make_uint4(0, 0, 0, 0);
+      if (k + 1 < lim) { nxt = ldg_stream16(next_row + lane * 16); ++rows_read; }
+      if (k < lim) {
+        const uint32_t nb = len - k * 16 < 16u ? len - k * 16 : 16u;
+        uint4 v = cur;
+#pragma unroll 1
+        for (uint32_t j = 0; j < nb; ++j) {                    // byte j of the row is the low byte of v.x
+          const uint32_t b = v.x & 0xFFu;
+          v.x = __funnelshift_r(v.x, v.y, 8); v.y = __funnelshift_r(v.y, v.z, 8); v.z = __funnelshift_r(v.z, v.w, 8); v.w >>= 8;
+          if constexpr (kHasDfa) d.step(b);
+          nfa.byte(t, b);
+        }
+      }
+      cur = nxt; row = next_row;
+      if (k + 1 < lim && decided()) lim = k + 1;               // row k + 1, already in flight, is dropped
+      if (__ballot_sync(0xffffffffu, k + 1 < lim) == 0) break;
+    }
+    if (live) {
+      uint32_t acc = nfa.finish(t);
+      if constexpr (kHasDfa) acc |= d.finish(endout);
+      a.hits[rec] = content_hits(acc, alive, queries, conds, nq);
+    } else if (rec != kInvalidRec && !a.has_alive) {
+      a.hits[rec] = 0;
+    }
+  }
+  unsigned long long bytes_read = 16ull * rows_read;
+  for (int o = 16; o; o >>= 1) bytes_read += __shfl_down_sync(0xffffffffu, bytes_read, o);
+  if (lane == 0 && touched) { atomicAdd(a.counter + 1, touched); atomicAdd(a.counter + 3, bytes_read); }
+}
+
+using BodyKernel = void (*)(BodyArgs);
+static BodyKernel body_nfa_kernel(uint32_t words, bool has_dfa) {
+  switch (words) {
+    case 1: return has_dfa ? k_body_nfa<1, true> : k_body_nfa<1, false>;
+    case 2: return has_dfa ? k_body_nfa<2, true> : k_body_nfa<2, false>;
+    case 4: return has_dfa ? k_body_nfa<4, true> : k_body_nfa<4, false>;
+    default: return has_dfa ? k_body_nfa<8, true> : k_body_nfa<8, false>;
+  }
+}
+static int body_nfa_threads(uint32_t words) { return words == 8 ? NfaThreads<8>::value : NfaThreads<4>::value; }
+
 // The content kernel of one scan: k_body_sticky when the sticky automaton's row addresses fit 16 bits, else the k_body
 // instance for the table's column mapping and accumulator mode.
-using BodyKernel = void (*)(BodyArgs);
 static BodyKernel body_kernel(bool sticky, bool direct, int acc_mode, bool push) {
   static const BodyKernel k_body_of[2][2][4] = {      // [push][direct][acc_mode]
       {{k_body<false, 0, false>, k_body<false, 1, false>, k_body<false, 2, false>, k_body<false, 3, false>},
@@ -1427,6 +1653,11 @@ template <typename Kernel, typename... Args>
 static int launch_body(Kernel k, unsigned grid, size_t smem, cudaStream_t s, Args... args) {
   FEI_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   k<<<grid, kBodyThreads, smem, s>>>(args...);
+  return FEI_OK;
+}
+static int launch_body_nfa(BodyKernel k, int threads, unsigned grid, size_t smem, cudaStream_t s, BodyArgs a) {
+  FEI_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  k<<<grid, threads, smem, s>>>(a);
   return FEI_OK;
 }
 
@@ -1553,7 +1784,8 @@ __global__ void __launch_bounds__(256) k_list_checksum(const T* __restrict__ v, 
 static int check_prog(const uint8_t* prog, uint64_t len) {
   if (!prog || len < sizeof(fei_prog_hdr)) { set_error("program blob too small"); return FEI_E_BADARG; }
   fei_prog_hdr h; memcpy(&h, prog, sizeof(h));
-  if (h.magic != FEI_PROG_MAGIC || h.version != FEI_PROG_VERSION) { set_error("bad program magic/version"); return FEI_E_BADARG; }
+  if (h.magic != FEI_PROG_MAGIC || (h.version != FEI_PROG_VERSION && h.version != FEI_PROG_VERSION_NFA) ||
+      (h.version == FEI_PROG_VERSION_NFA) != (h.off_body_nfa != 0)) { set_error("bad program magic/version"); return FEI_E_BADARG; }
   if (h.total_bytes != len) { set_error("program length mismatch (%u vs %llu)", h.total_bytes, (unsigned long long)len); return FEI_E_BADARG; }
   if (h.n_queries == 0 || h.n_queries > FEI_MAX_QUERIES) { set_error("1..32 queries per program"); return FEI_E_BADARG; }
   if (h.n_slots > FEI_MAX_SLOTS) { set_error("at most %d header slots per program", FEI_MAX_SLOTS); return FEI_E_UNSUPPORTED; }
@@ -1575,6 +1807,32 @@ static int check_prog(const uint8_t* prog, uint64_t len) {
   const fei_prog_slot* sl = reinterpret_cast<const fei_prog_slot*>(prog + h.off_slots);
   for (uint32_t s = 0; s < h.n_slots; ++s) if (!sl[s].off_val_dfa || !dfa_ok(sl[s].off_val_dfa)) { set_error("bad slot DFA"); return FEI_E_BADARG; }
   if (h.n_slots && !h.off_key_dfa) { set_error("slots without a key DFA"); return FEI_E_BADARG; }
+  if (h.off_body_nfa) {                            // the content position automaton: every table inside its table_bytes
+    if (!in(h.off_body_nfa, sizeof(fei_prog_nfa))) { set_error("content position automaton out of bounds"); return FEI_E_BADARG; }
+    fei_prog_nfa a; memcpy(&a, prog + h.off_body_nfa, sizeof(a));
+    const uint64_t W = a.n_words, end = (uint64_t)a.off_ascii + a.table_bytes;
+    auto tab = [&](uint64_t off, uint64_t sz) { return off % 16 == 0 && off >= a.off_ascii && off + sz <= end; };
+    bool ok = (W == 1 || W == 2 || W == 4 || W == 8) && a.n_pos >= 1 && a.n_pos <= 32 * W && a.n_classes >= 1 &&
+              a.n_classes <= FEI_NFA_MAX_CLASSES && a.n_ranges >= 1 && a.n_ranges <= FEI_NFA_MAX_RANGES &&
+              a.n_follow <= FEI_NFA_MAX_GROUPS && a.n_accept <= FEI_NFA_MAX_GROUPS && a.first_bit + (uint64_t)a.n_patterns <= 32 &&
+              a.table_bytes % 16 == 0 && in(a.off_ascii, a.table_bytes) && tab(a.off_ascii, 2 * 128) &&
+              tab(a.off_range_lo, 4ull * a.n_ranges) && tab(a.off_range_ck, 2ull * a.n_ranges) && tab(a.off_cls_b, 4ull * W * a.n_classes) &&
+              tab(a.off_masks, 12ull * W) && tab(a.off_follow, 4ull * (2 * W + 1) * a.n_follow) && tab(a.off_accept, 4ull * (W + 2) * a.n_accept);
+    if (ok) {                                      // class ids index cls_b, kinds are 0..4, the range table starts at 0x80
+      const uint16_t* asc = reinterpret_cast<const uint16_t*>(prog + a.off_ascii);
+      const uint16_t* rck = reinterpret_cast<const uint16_t*>(prog + a.off_range_ck);
+      const uint32_t* rlo = reinterpret_cast<const uint32_t*>(prog + a.off_range_lo);
+      auto ck_ok = [&](uint16_t v) { return (v & 0xFFu) < a.n_classes && (v >> 8) < 5; };
+      for (int c = 0; c < 128 && ok; ++c) ok = ck_ok(asc[c]);
+      for (uint32_t r = 0; r < a.n_ranges && ok; ++r) ok = ck_ok(rck[r]) && (r ? rlo[r] > rlo[r - 1] : rlo[0] == 0x80u);
+      const uint32_t* acc = reinterpret_cast<const uint32_t*>(prog + a.off_accept);
+      for (uint32_t g = 0; g < a.n_accept && ok; ++g) ok = (acc[g * (W + 2) + W + 1] & 0xFFu) < 32;
+    }
+    if (!ok) { set_error("bad content position automaton in program"); return FEI_E_BADARG; }
+    fei_prog_dfa d{};
+    if (h.off_body_dfa) memcpy(&d, prog + h.off_body_dfa, sizeof(d));
+    if (h.off_body_dfa && (d.n_cols == 256 || d.sticky || d.table_bytes % 16)) { set_error("the body DFA next to a position automaton must be class-indexed"); return FEI_E_BADARG; }
+  }
   if (h.head_bytes > h.total_bytes || (h.head_bytes & 15u)) { set_error("bad head_bytes in program"); return FEI_E_BADARG; }
   const fei_prog_query* qs = reinterpret_cast<const fei_prog_query*>(prog + h.off_queries);
   for (uint32_t q = 0; q < h.n_queries; ++q) if (qs[q].cond_begin > qs[q].cond_end || qs[q].cond_end > h.n_conds) { set_error("bad query range"); return FEI_E_BADARG; }
@@ -1604,7 +1862,8 @@ int run_scan(fei_corpus* c, const uint8_t* prog, uint64_t prog_len, int compact_
   FEI_CUDA(cudaMemcpyAsync(c->prog.p, prog, prog_len, cudaMemcpyHostToDevice, s));
   FEI_CUDA(cudaMemsetAsync(c->work_counter.p, 0, kWorkCounters * sizeof(unsigned long long), s));
   bool need_head = h.head_mask != 0;
-  bool need_body = h.off_body_dfa != 0 && h.body_mask != 0;
+  bool need_body = (h.off_body_dfa != 0 || h.off_body_nfa != 0) && h.body_mask != 0;
+  const bool nfa = need_body && h.off_body_nfa != 0;           // k_body_nfa (with the body DFA, if any, stepped alongside)
   if ((h.off_name_dfa[0] || h.off_name_dfa[1] || h.off_name_dfa[2]) && !c->name.p) {
     set_error("program reads filename / id / hostname but the corpus was packed without names"); return FEI_E_STATE;
   }
@@ -1682,7 +1941,15 @@ int run_scan(fei_corpus* c, const uint8_t* prog, uint64_t prog_len, int compact_
   fei_prog_dfa d; memset(&d, 0, sizeof(d));
   size_t smem = 0;
   int acc_mode = 0; bool direct = false, sticky_kernel = false, gather = false;
-  if (n && need_body) {
+  fei_prog_nfa na; memset(&na, 0, sizeof(na));
+  if (n && nfa) {
+    if (h.off_body_dfa) memcpy(&d, prog + h.off_body_dfa, sizeof(d));
+    memcpy(&na, prog + h.off_body_nfa, sizeof(na));
+    smem = (size_t)d.table_bytes + na.table_bytes;
+    if (smem > 220 * 1024) { set_error("content automata need %zu bytes of shared memory (limit 220 KiB)", smem); return FEI_E_UNSUPPORTED; }
+    c->timing.body_kernel = 4u;
+    c->timing.body_nfa_words = na.n_words;
+  } else if (n && need_body) {
     memcpy(&d, prog + h.off_body_dfa, sizeof(d));
     smem = d.table_bytes;
     if (smem > 220 * 1024) { set_error("content automaton needs %zu bytes of shared memory (limit 220 KiB)", smem); return FEI_E_UNSUPPORTED; }
@@ -1703,9 +1970,10 @@ int run_scan(fei_corpus* c, const uint8_t* prog, uint64_t prog_len, int compact_
   const uint64_t n_windows = (n + kWindow - 1) / kWindow;
   // k_body (every multi-pattern scan, and single-pattern ones the sticky kernel cannot take) builds the ordered lists inside the
   // scan; the other scans compact the finished masks with k_count / k_scan_blocks / k_emit after it
-  const bool body_lists = n && need_body && !sticky_kernel && compact_mode == kCompactLists;
-  // multi-GPU: the scan kernel stores every finished window's masks into the peers (k_body_gather does not: the hook copies them)
-  const bool push = n && need_body && !gather && hook && hook->push_peers && hook->push_n;
+  const bool body_lists = n && need_body && !nfa && !sticky_kernel && compact_mode == kCompactLists;
+  // multi-GPU: the scan kernel stores every finished window's masks into the peers (k_body_gather and k_body_nfa do not: the
+  // hook copies them)
+  const bool push = n && need_body && !nfa && !gather && hook && hook->push_peers && hook->push_n;
   BodyArgs a{c->prog.as<uint8_t>(), c->tiles.as<uint8_t>(), c->grp_base.as<uint64_t>(), c->grp_rec.as<uint32_t>(), c->grp_len.as<uint32_t>(),
              c->n_groups, c->hits.as<uint32_t>(), need_head ? 1 : 0, c->work_counter.as<unsigned long long>(), 0ull,
              c->work_counter.as<unsigned long long>(), nullptr};
@@ -1731,7 +1999,10 @@ int run_scan(fei_corpus* c, const uint8_t* prog, uint64_t prog_len, int compact_
     a.totals = c->compact.totals.as<unsigned long long>(); a.nq = nq;
   }
   if (push) { a.push_peers = hook->push_peers; a.push_n = hook->push_n; a.push_off = hook->push_off; hook->pushed = true; }
-  if (n && need_body) {
+  if (n && nfa) {
+    FEI_TRY(launch_body_nfa(body_nfa_kernel(na.n_words, h.off_body_dfa != 0), body_nfa_threads(na.n_words), grid, smem, s, a));
+    ++launches;
+  } else if (n && need_body) {
     const size_t body_smem = sticky_kernel ? ((smem + 127) & ~(size_t)127) + kStickyRingBytes : smem;   // k_body_sticky: + its rings
     FEI_TRY(launch_body(body_kernel(sticky_kernel, direct, acc_mode, a.push_n != 0), grid, body_smem, s, a));
     ++launches;

@@ -20,7 +20,7 @@ import numpy as np
 
 from .. import packer
 from ..program import (C_BODY, C_CONST, C_DATE_CMP, C_FLAGS, C_FOLDER_SET, C_NAME, C_RECBITS, C_SLOT, C_STATUS_SET, C_TS_CMP, CMP, MAX_AUX,
-                       NAME_DATE_STR, NAME_FILENAME, NAME_HOST, NAME_ID, NAME_TS_STR, Cond, ProgramBuilder, const)
+                       NAME_DATE_STR, NAME_FILENAME, NAME_HOST, NAME_ID, NAME_TS_STR, Cond, ProgramBuilder, const, content_automaton)
 from ..regexc import Pattern, compile_patterns
 from . import utils as U
 
@@ -198,7 +198,7 @@ def _compile_one(field: Any, op: str, v2: Any, include_content: bool, pm) -> Lis
         if isinstance(pat, Exception):
             return [_Raises(pat, None)]
         if not include_content:                                           # memory.get("content", "") == "" (search.py:103-104, :363)
-            return [const(bool(compile_patterns([pat]).run(b"") & 1) != neg)]
+            return [const(bool(content_automaton(pat).run(b"") & 1) != neg)]
         return [Cond(C_BODY, pattern=pat, negate=neg)]
     if low == "flags":
         pat, neg = _string_pattern(op, v2, "flags")

@@ -12,14 +12,15 @@ from typing import Dict, List, Optional, Sequence, Tuple
 
 import numpy as np
 
-from .regexc import Dfa, Pattern, compile_patterns
+from .regexc import Dfa, Pattern, PatternTooLarge, Pna, compile_patterns, compile_positions
 
-MAGIC, VERSION = 0x50494546, 1
+MAGIC, VERSION, VERSION_NFA = 0x50494546, 1, 2
 C_CONST, C_BODY, C_SLOT, C_FLAGS, C_NAME, C_DATE_CMP, C_FOLDER_SET, C_STATUS_SET, C_RECBITS, C_TS_CMP = range(10)
 CMP = {">": 0, "<": 1, ">=": 2, "<=": 3, "=": 4, "!=": 5}
 NAME_FILENAME, NAME_ID, NAME_HOST, NAME_TS_STR, NAME_DATE_STR = 0, 1, 2, 3, 4     # 3 / 4: str(metadata["timestamp"]) / str(metadata["date"]), formatted by the kernels
 MAX_AUX = 4                            # aux verdict columns per corpus (FEI_C_RECBITS)
 SMEM_TABLE_LIMIT = 200 * 1024          # body automaton must fit the CTA's shared memory
+BODY_SMEM_LIMIT = 220 * 1024           # scan.cu: dynamic shared memory of a body kernel (content DFA + position automaton tables)
 HEAD_SMEM_WINDOW = 32 * 1024           # scan.cu kHeadProgSmem: the program head the head kernels stage per CTA
 HEAD_DIRECT_LIMIT = 12 * 1024          # a head automaton up to this size is stored byte-indexed
 
@@ -54,6 +55,56 @@ def _pad16(b: bytearray) -> None:
 
 
 _DFA_CACHE: Dict[Tuple, Dfa] = {}
+_DFA_FAIL: Dict[Tuple, str] = {}       # same keys: pattern sets whose DFA was refused (PatternTooLarge), with the reason
+_PNA_CACHE: Dict[Tuple, Pna] = {}
+
+
+def _remember(cache: Dict, key, value) -> None:
+    if len(cache) >= 256:
+        cache.pop(next(iter(cache)))
+    cache[key] = value
+
+
+def _pkey(p: Pattern) -> Tuple:
+    return (p.kind, p.text, int(p.flags))
+
+
+def cached_dfa(patterns: Sequence[Pattern], sticky: bool = False) -> Dfa:
+    """compile_patterns, cached per process; a refusal (PatternTooLarge) is cached too, so a repeated query does not pay for
+    the failed subset construction again (seconds for a bounded gap such as `.{0,60}`)."""
+    sticky = sticky and len(patterns) == 1
+    key = (tuple(_pkey(p) for p in patterns), sticky)
+    d = _DFA_CACHE.get(key)
+    if d is not None:
+        return d
+    why = _DFA_FAIL.get(key)
+    if why is not None:
+        raise PatternTooLarge(why)
+    try:
+        d = compile_patterns(patterns, sticky=sticky)
+    except PatternTooLarge as e:
+        _remember(_DFA_FAIL, key, str(e))
+        raise
+    _remember(_DFA_CACHE, key, d)
+    return d
+
+
+def cached_positions(patterns: Sequence[Pattern]) -> Pna:
+    key = tuple(_pkey(p) for p in patterns)
+    a = _PNA_CACHE.get(key)
+    if a is None:
+        a = compile_positions(patterns)
+        _remember(_PNA_CACHE, key, a)
+    return a
+
+
+def content_automaton(p: Pattern):
+    """The automaton a `content` condition runs: its DFA, or its position automaton when the DFA is refused.  Both have
+    .run(bytes) -> mask (the empty-string verdict of a content condition without with_content)."""
+    try:
+        return cached_dfa([p])
+    except PatternTooLarge:
+        return cached_positions([p])
 
 
 class _FieldDfa:
@@ -78,15 +129,7 @@ class _FieldDfa:
     def compile(self, sticky: bool = False) -> Dfa:
         """Compiled automata are cached per process: repeated queries / the default filters skip the (host-side,
         Python) subset construction, which costs 10-900 ms for Unicode-class-heavy patterns."""
-        sticky = sticky and len(self.patterns) == 1
-        key = (tuple((p.kind, p.text, int(p.flags)) for p in self.patterns), sticky)
-        d = _DFA_CACHE.get(key)
-        if d is None:
-            d = compile_patterns(self.patterns, sticky=sticky)
-            if len(_DFA_CACHE) >= 256:
-                _DFA_CACHE.pop(next(iter(_DFA_CACHE)))
-            _DFA_CACHE[key] = d
-        return d
+        return cached_dfa(self.patterns, sticky)
 
 
 def tile_byte_perm(b: np.ndarray) -> np.ndarray:
@@ -150,6 +193,89 @@ def serialize_dfa(d: Dfa, blob: bytearray, direct_limit: int = 0, tile_bytes: bo
     return desc_off
 
 
+def _table_bytes(d: Dfa, direct_limit: int) -> int:
+    """fei_prog_dfa.table_bytes that serialize_dfa(d, blob, direct_limit) writes, without writing it."""
+    n = d.n_states
+    ncols = 256 if direct_limit and n * 516 + n * 8 + 256 <= direct_limit else d.ctrans.shape[1]
+    stride = ncols + (ncols & 1)
+    if (stride // 2) % 2 == 0:
+        stride += 2
+    return sum((x + 15) & ~15 for x in (2 * n * stride, 4 * n, 4 * n, 256))
+
+
+def serialize_nfa(a: Pna, blob: bytearray, first_bit: int) -> int:
+    """Append a fei_prog_nfa section (include/feiscan_prog.h); returns its offset.  Output bit k of the automaton becomes
+    content bit first_bit + k."""
+    W = a.n_words
+    if first_bit + a.n_patterns > 32:
+        raise NotImplementedError("more than 32 content patterns in one program")
+
+    def words(m: int) -> List[int]:
+        return [(m >> (32 * k)) & 0xFFFFFFFF for k in range(W)]
+
+    def table(arr: np.ndarray) -> int:
+        off = len(blob)
+        blob.extend(arr.tobytes()); _pad16(blob)
+        return off
+
+    _pad16(blob)
+    desc_off = len(blob)
+    blob.extend(b"\0" * 64)
+    ck = lambda c: c | a.cls_kind[c] << 8                                          # noqa: E731
+    off_ascii = table(np.array([ck(c) for c in a.ascii_cls], dtype=np.uint16))
+    off_lo = table(np.array([lo for lo, _c in a.ranges], dtype=np.uint32))
+    off_rck = table(np.array([ck(c) for _lo, c in a.ranges], dtype=np.uint16))
+    off_b = table(np.array([w for b in a.cls_b for w in words(b)], dtype=np.uint32))
+    off_masks = table(np.array(words(a.shift) + words(a.self_loop) + words(a.start), dtype=np.uint32))
+    off_follow = table(np.array([w for src, dst, m in a.follow for w in words(src) + words(dst) + [m]], dtype=np.uint32))
+    off_accept = table(np.array([w for src, m, p, eo in a.accept for w in words(src) + [m, (first_bit + p) | (int(eo) << 8)]],
+                                dtype=np.uint32))
+    struct.pack_into("<16I", blob, desc_off, W, a.n_pos, len(a.cls_b), len(a.ranges), len(a.follow), len(a.accept), a.n_patterns,
+                     first_bit, off_ascii, off_lo, off_rck, off_b, off_masks, off_follow, off_accept, len(blob) - off_ascii)
+    return desc_off
+
+
+def _route_body(patterns: Sequence[Pattern]) -> Tuple[List[int], List[int], Optional[Pna]]:
+    """Which content patterns the body DFA takes and which go to the position automaton: (dfa indices, nfa indices, the
+    automaton of the nfa ones).  The union goes to the DFA whenever it compiles and fits, exactly as without the position
+    automaton.  Otherwise every pattern whose DFA is refused on its own goes to the position automaton, and then the
+    patterns with the largest DFAs until the union of the rest fits next to the position automaton's tables."""
+    idx = list(range(len(patterns)))
+    try:
+        if _table_bytes(cached_dfa(patterns, sticky=True), SMEM_TABLE_LIMIT) <= BODY_SMEM_LIMIT:
+            return idx, [], None
+    except PatternTooLarge:
+        pass
+    size: Dict[int, int] = {}
+    for i in idx:
+        try:
+            d = cached_dfa([patterns[i]])
+            if _table_bytes(d, 0) <= BODY_SMEM_LIMIT:
+                size[i] = d.n_states
+        except PatternTooLarge:
+            pass
+    dfa = [i for i in idx if i in size]
+    while True:
+        nfa = [i for i in idx if i not in dfa]
+        a = cached_positions([patterns[i] for i in nfa])
+        room = BODY_SMEM_LIMIT - _nfa_table_bytes(a)
+        if not dfa:
+            break
+        try:
+            if _table_bytes(cached_dfa([patterns[i] for i in dfa]), 0) <= room:
+                break
+        except PatternTooLarge:
+            pass
+        dfa.remove(max(dfa, key=lambda i: (size[i], i)))
+    return dfa, nfa, a
+
+
+def _nfa_table_bytes(a: Pna) -> int:
+    scratch = bytearray()
+    off = serialize_nfa(a, scratch, 0)
+    return struct.unpack_from("<I", scratch, off + 60)[0]
+
+
 class ProgramBuilder:
     def __init__(self):
         self.queries: List[List[Cond]] = []
@@ -202,6 +328,12 @@ class ProgramBuilder:
                         ref = c.which
                 recs.append((c.kind, ref, bit, 1 if c.negate else 0, c.if_missing, c.op, c.i64, c.set64))
             qranges.append((begin, len(recs)))
+        # content patterns too large for the body DFA go to the position automaton; content bits are renumbered so that the
+        # DFA's outputs come first and the position automaton's follow
+        body_dfa, body_nfa, pna = _route_body(body.patterns) if body.patterns else ([], [], None)
+        if body_nfa:
+            new_bit = {old: new for new, old in enumerate(body_dfa + body_nfa)}
+            recs = [(kind, ref, new_bit[bit] if kind == C_BODY else bit, *rest) for kind, ref, bit, *rest in recs]
 
         # small head automata are stored byte-indexed (one lookup per byte in the head kernels) as long as the whole
         # program head still fits the kernels' shared-memory window; otherwise class-indexed (two lookups, smaller)
@@ -232,15 +364,23 @@ class ProgramBuilder:
             if len(blob) <= HEAD_SMEM_WINDOW:
                 break
         head_bytes = len(blob)               # the content automaton goes last: [0, head_bytes) is what the head kernels stage
-        off_body = serialize_dfa(body.compile(sticky=True), blob, SMEM_TABLE_LIMIT, tile_bytes=True) if body.patterns else 0
-        if off_body:
-            tb = struct.unpack_from("<I", blob, off_body + 44)[0]
-            if tb > 220 * 1024:
-                raise NotImplementedError(f"content automaton needs {tb} bytes of shared memory (limit 220 KiB)")
+        off_nfa = 0
+        if not body_nfa:
+            off_body = serialize_dfa(body.compile(sticky=True), blob, SMEM_TABLE_LIMIT, tile_bytes=True) if body.patterns else 0
+        else:                                # the DFA part class-indexed: k_body_nfa steps one DFA variant
+            dfa_pats = [body.patterns[i] for i in body_dfa]
+            off_body = serialize_dfa(cached_dfa(dfa_pats), blob, 0, tile_bytes=True) if dfa_pats else 0
+            off_nfa = serialize_nfa(pna, blob, len(dfa_pats))
+        tb = struct.unpack_from("<I", blob, off_body + 44)[0] if off_body else 0
+        if off_nfa:
+            tb = tb + struct.unpack_from("<I", blob, off_nfa + 60)[0]
+        if tb > BODY_SMEM_LIMIT:
+            raise NotImplementedError(f"content automaton needs {tb} bytes of shared memory (limit 220 KiB)")
         _pad16(blob)
-        struct.pack_into("<22I", blob, 0, MAGIC, VERSION, len(blob), len(self.queries), len(recs), off_conds, off_queries,
-                         len(slots), off_slots, off_key, off_body, off_flags, off_names[0], off_names[1], off_names[2],
+        struct.pack_into("<22I", blob, 0, MAGIC, VERSION_NFA if off_nfa else VERSION, len(blob), len(self.queries), len(recs), off_conds,
+                         off_queries, len(slots), off_slots, off_key, off_body, off_flags, off_names[0], off_names[1], off_names[2],
                          head_mask, body_mask, slot_mask, name_mask, head_bytes, off_names[3], off_names[4])
+        struct.pack_into("<I", blob, 88, off_nfa)
         return bytes(blob)
 
 

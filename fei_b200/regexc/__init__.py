@@ -926,3 +926,234 @@ def _byte_classes(d: Dfa) -> None:
     cols, inv = np.unique(d.trans, axis=1, return_inverse=True)
     d.cls = inv.reshape(-1).astype(np.uint8)
     d.ctrans = np.ascontiguousarray(cols)
+
+
+# --------------------------------------------------------------------------- position automaton (bit-parallel NFA)
+# For patterns whose DFA is too large (bounded gaps such as `a.{0,60}b` remember every recent start: the subset construction
+# grows exponentially in the gap), the scan steps the NFA itself as a bit vector over its character edges ("positions",
+# Glushkov form): every edge into position j consumes a code point of leaf(j), so one step is
+#     D' = Follow(D, ctx) & B[class(c)]
+#     Follow(D, ctx) = ((D << 1) & SHIFT) | (D & SELF) | OR_g [(D & SRC_g) != 0 and ctx in CTX_g] DST_g
+# Assertions only read the code points on both sides of a boundary, so an epsilon path is valid under a set of
+# (previous kind, next kind) context pairs: 5 kinds x 5 kinds = 25 bits.
+K_EDGE, K_NL, K_WORD, K_UWORD, K_OTHER = range(5)     # start/end sentinel, '\n', \w in both senses, Unicode-only \w, other
+N_KINDS = 5
+CTX_ALL = (1 << (N_KINDS * N_KINDS)) - 1
+PNA_MAX_POS = 256            # bits of the position vector, the virtual start bit included (8 words of 32)
+PNA_MAX_CLASSES = 128
+PNA_MAX_RANGES = 4096        # non-ASCII code point ranges (binary-searched in shared memory)
+PNA_MAX_FOLLOW = 64
+PNA_MAX_ACCEPT = 64
+
+
+def ctx_bit(prev_kind: int, next_kind: int) -> int:
+    return 1 << (prev_kind * N_KINDS + next_kind)
+
+
+_PREV_CTX = {K_EDGE: (2, 0, 0), K_NL: (1, 0, 0), K_WORD: (0, 1, 1), K_UWORD: (0, 1, 0), K_OTHER: (0, 0, 0)}
+_NEXT_CTX = {**_PREV_CTX, K_EDGE: (3, 0, 0)}
+
+
+def _cond_ok(cond: int, prev, nxt) -> bool:
+    """`cond_ok` of _determinize: prev / nxt are (nl: 0/1, 2 = start, 3 = end; uword; aword)."""
+    if cond == A_BOS:
+        return prev[0] == 2
+    if cond == A_BOL:
+        return prev[0] == 2 or prev[0] == 1
+    if cond == A_EOS:
+        return nxt[0] == 3
+    if cond == A_EOL:
+        return nxt[0] == 3 or nxt[0] == 1
+    if cond == A_NEXTNL:
+        return nxt[0] == 1
+    if prev[0] == 2 and nxt[0] == 3:
+        return False
+    k = 1 if cond in (A_WB_U, A_NWB_U) else 2
+    pw = prev[k] if prev[0] != 2 else 0
+    nw = nxt[k] if nxt[0] != 3 else 0
+    return (pw != nw) if cond in (A_WB_U, A_WB_A) else (pw == nw)
+
+
+@dataclass
+class Pna:
+    """Position automaton of a pattern set.  Bit 0 is the virtual start position (set before the first character only);
+    bit i >= 1 is character edge i of the NFA.  Masks are Python ints over n_pos bits."""
+    n_words: int
+    n_pos: int
+    n_patterns: int
+    ascii_cls: List[int]                      # [128] class of each ASCII code point
+    ranges: List[Tuple[int, int]]             # sorted (first code point, class), covering 0x80 .. 0x10FFFF
+    cls_b: List[int]                          # [class] positions whose leaf holds the class
+    cls_kind: List[int]                       # [class] context kind
+    shift: int
+    self_loop: int
+    start: int
+    follow: List[Tuple[int, int, int]]        # (src, dst, ctx mask)
+    accept: List[Tuple[int, int, int, bool]]  # (src, ctx mask, pattern, end only)
+
+    def cls_of(self, cp: int) -> int:
+        if cp < 0x80:
+            return self.ascii_cls[cp]
+        lo, hi = 0, len(self.ranges) - 1
+        while lo < hi:
+            mid = (lo + hi + 1) >> 1
+            if self.ranges[mid][0] <= cp:
+                lo = mid
+            else:
+                hi = mid - 1
+        return self.ranges[lo][1]
+
+    def follow_of(self, d: int, ctx: int) -> int:
+        nd = ((d << 1) & self.shift) | (d & self.self_loop)
+        for src, dst, m in self.follow:
+            if m & ctx and d & src:
+                nd |= dst
+        return nd
+
+    def accepts(self, d: int, ctx: int, at_end: bool) -> int:
+        acc = 0
+        for src, m, p, end_only in self.accept:
+            if (at_end or not end_only) and m & ctx and d & src:
+                acc |= 1 << p
+        return acc
+
+    def run(self, data: bytes) -> int:
+        """Host simulation: mask of matching patterns for `data` (valid UTF-8), like Dfa.run."""
+        d, prev, acc = self.start, K_EDGE, 0
+        for ch in data.decode("utf-8", "surrogatepass"):
+            c = self.cls_of(ord(ch))
+            kind = self.cls_kind[c]
+            ctx = ctx_bit(prev, kind)
+            acc |= self.accepts(d, ctx, False)
+            d = self.follow_of(d, ctx) & self.cls_b[c]
+            prev = kind
+        return acc | self.accepts(d, ctx_bit(prev, K_EDGE), True)
+
+
+def _positions(n: Nfa) -> List[Tuple[int, int, int]]:
+    """Character edges (src, leaf, dst) reachable from the start, numbered depth-first with a state's character edges
+    before its epsilon edges, so that a chain of characters gets consecutive numbers (follow edge i -> i + 1)."""
+    out: List[Tuple[int, int, int]] = []
+    seen = {n.start}
+    stack = [(n.start, iter([("c", e) for e in n.chars[n.start]] + [("e", e) for e in n.eps[n.start]]))]
+    while stack:
+        s, it = stack[-1]
+        nxt = next(it, None)
+        if nxt is None:
+            stack.pop()
+            continue
+        kind, e = nxt
+        if kind == "c":
+            leaf, d = e
+            out.append((s, leaf, d))
+        else:
+            d = e[0]
+        if d not in seen:
+            seen.add(d)
+            stack.append((d, iter([("c", x) for x in n.chars[d]] + [("e", x) for x in n.eps[d]])))
+    return out
+
+
+def compile_positions(patterns: Sequence[Pattern]) -> Pna:
+    """Pattern set -> position automaton (pattern k = output bit k), from the same NFA compile_patterns determinizes."""
+    if len(patterns) > 32:
+        raise ValueError("at most 32 patterns per automaton")
+    n = Nfa()
+    for pid, p in enumerate(patterns):
+        add_pattern(n, pid, p)
+    n.add_trailing_newline_rule()
+    pos = _positions(n)
+    n_pos = len(pos) + 1
+    if n_pos > PNA_MAX_POS:
+        raise PatternTooLarge(f"position automaton needs {n_pos} bits (limit {PNA_MAX_POS})")
+    # code point classes: the leaves of the positions, plus the sets that decide a class' context kind
+    uses = n.uses
+    need_nl = A_BOL in uses or A_EOL in uses or A_NEXTNL in uses
+    need_uw = bool(uses & {A_WB_U, A_NWB_U, A_WB_A, A_NWB_A})
+    leaf_ids = sorted({leaf for _s, leaf, _d in pos})
+    leaves = [n.leaves[x] for x in leaf_ids]
+    ctx_leaf = {}
+    if need_nl:
+        ctx_leaf["nl"] = len(leaves); leaves.append(_NL)
+    if need_uw:
+        ctx_leaf["uw"] = len(leaves); leaves.append(_uword_set())
+        ctx_leaf["aw"] = len(leaves); leaves.append(_AWORD)
+    bounds, cls_of, members = _partition(leaves)
+    ncls = len(members)
+    if ncls > PNA_MAX_CLASSES:
+        raise PatternTooLarge(f"position automaton needs {ncls} code point classes (limit {PNA_MAX_CLASSES})")
+
+    def has(m, name):
+        return name in ctx_leaf and (m >> ctx_leaf[name]) & 1
+
+    kinds = [K_NL if has(m, "nl") else K_WORD if has(m, "aw") else K_UWORD if has(m, "uw") else K_OTHER for m in members]
+    col = {leaf: k for k, leaf in enumerate(leaf_ids)}
+    cls_b = [0] * ncls
+    for i, (_s, leaf, _d) in enumerate(pos):
+        bit = 1 << col[leaf]
+        for c in range(ncls):
+            if members[c] & bit:
+                cls_b[c] |= 1 << (i + 1)
+    ascii_cls = [int(cls_of[np.searchsorted(bounds, cp, side="right") - 1]) for cp in range(0x80)]
+    ranges: List[Tuple[int, int]] = []
+    for j in range(len(bounds) - 1):
+        lo = int(bounds[j])
+        if lo > MAX_CP:
+            break
+        lo = max(lo, 0x80)
+        if int(bounds[j + 1]) <= lo:
+            continue
+        c = int(cls_of[j])
+        if not ranges or ranges[-1][1] != c:
+            ranges.append((lo, c))
+    if len(ranges) > PNA_MAX_RANGES:
+        raise PatternTooLarge(f"position automaton needs {len(ranges)} code point ranges (limit {PNA_MAX_RANGES})")
+
+    # epsilon closures of every position's location under each of the 25 context pairs
+    src_of: Dict[int, List[int]] = {}
+    for i, (s, _leaf, _d) in enumerate(pos):
+        src_of.setdefault(s, []).append(i + 1)
+    locs = [n.start] + [d for _s, _leaf, d in pos]
+    ctxs = [(pk, nk, ctx_bit(pk, nk), _PREV_CTX[pk], _NEXT_CTX[nk]) for pk in range(N_KINDS) for nk in range(N_KINDS)]
+    shift = self_loop = 0
+    follow: Dict[Tuple[int, int], int] = {}          # (dst set, ctx mask) -> src set
+    accept: Dict[Tuple[int, int, bool], int] = {}    # (ctx mask, pattern, end only) -> src set
+    for i, q in enumerate(locs):
+        fm: Dict[int, int] = {}                      # position j -> ctx mask
+        am: Dict[int, int] = {}                      # accepting state -> ctx mask
+        for _pk, _nk, cb, pt, nt in ctxs:
+            seen = {q}
+            stack = [q]
+            while stack:
+                s = stack.pop()
+                for dst, cond in n.eps[s]:
+                    if dst not in seen and (cond == 0 or _cond_ok(cond, pt, nt)):
+                        seen.add(dst); stack.append(dst)
+            for s in seen:
+                for j in src_of.get(s, ()):
+                    fm[j] = fm.get(j, 0) | cb
+                if s in n.accept:
+                    am[s] = am.get(s, 0) | cb
+        by_mask: Dict[int, int] = {}
+        for j, m in fm.items():
+            if m == CTX_ALL and j == i + 1:
+                shift |= 1 << j
+            elif m == CTX_ALL and j == i:
+                self_loop |= 1 << j
+            else:
+                by_mask[m] = by_mask.get(m, 0) | (1 << j)
+        for m, dst in by_mask.items():
+            follow[(dst, m)] = follow.get((dst, m), 0) | (1 << i)
+        for s, m in am.items():
+            key = (m, n.accept[s], s in n.end_only)
+            accept[key] = accept.get(key, 0) | (1 << i)
+    if len(follow) > PNA_MAX_FOLLOW or len(accept) > PNA_MAX_ACCEPT:
+        raise PatternTooLarge(f"position automaton needs {len(follow)} follow and {len(accept)} accept groups "
+                              f"(limits {PNA_MAX_FOLLOW} / {PNA_MAX_ACCEPT})")
+    words = 1
+    while words * 32 < n_pos:
+        words *= 2
+    return Pna(n_words=words, n_pos=n_pos, n_patterns=len(patterns), ascii_cls=ascii_cls, ranges=ranges, cls_b=cls_b,
+               cls_kind=kinds, shift=shift, self_loop=self_loop, start=1,
+               follow=[(src, dst, m) for (dst, m), src in follow.items()],
+               accept=[(src, m, p, eo) for (m, p, eo), src in accept.items()])

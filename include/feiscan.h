@@ -236,13 +236,15 @@ typedef struct fei_scan_timing {
   uint64_t body_bytes_read;      /* tile bytes the body kernel really requested (a multi-pattern scan stops reading a
                                     record once its content verdicts are decided, a single-pattern scan stops reading a
                                     group once all of its records have matched; copies already in flight are counted) */
-  uint32_t body_kernel;          /* 0 no content pass, 1 k_body_sticky, 2 k_body_gather, 3 k_body.  The sticky / gather choice
-                                    is made on the device from the records left alive by the header conditions: 2 when at most
-                                    1 in 16 are; also 2 when none is, in which case neither kernel reads a byte
-                                    (body_bytes_read == 0) */
+  uint32_t body_kernel;          /* 0 no content pass, 1 k_body_sticky, 2 k_body_gather, 3 k_body, 4 k_body_nfa (content patterns
+                                    too large for the DFA run as a position automaton, next to the DFA of the others).  The
+                                    sticky / gather choice is made on the device from the records left alive by the header
+                                    conditions: 2 when at most 1 in 16 are; also 2 when none is, in which case neither kernel
+                                    reads a byte (body_bytes_read == 0) */
   uint32_t body_direct;          /* content automaton rows: 1 byte-indexed, 0 class-indexed */
   uint32_t body_acc_mode;        /* how k_body records accepting states: 1 / 2 <= 32 / <= 64 of them as register bits,
                                     0 out[] per step, 3 single-pattern (sticky) automaton */
+  uint32_t body_nfa_words;       /* k_body_nfa: 32-bit words per position vector (1, 2, 4 or 8); 0 for the other kernels */
 } fei_scan_timing;
 int fei_scan_last_timing(const fei_corpus* c, fei_scan_timing* out);
 

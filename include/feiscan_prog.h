@@ -18,6 +18,7 @@
 
 #define FEI_PROG_MAGIC   0x50494546u   /* "FEIP" */
 #define FEI_PROG_VERSION 1u
+#define FEI_PROG_VERSION_NFA 2u        /* written only by programs that carry a content position automaton (fei_prog_nfa) */
 #define FEI_MAX_QUERIES  32
 #define FEI_MAX_SLOTS    16
 
@@ -59,8 +60,35 @@ typedef struct fei_prog_hdr {            /* 96 bytes */
   uint32_t head_bytes;                   /* everything before the content automaton (which is serialised last): the part the
                                             head kernels copy into shared memory; 0 = unknown (do not stage)              */
   uint32_t off_meta_dfa[2];              /* name fields 3 and 4: automata over the formatted timestamp / date strings        */
-  uint32_t reserved[2];
+  uint32_t off_body_nfa;                 /* version 2 only: fei_prog_nfa of the content patterns too large for the body DFA; 0 = none */
+  uint32_t reserved;
 } fei_prog_hdr;
+
+/* Content position automaton (bit-parallel NFA, fei_b200/regexc compile_positions), for content patterns whose DFA is too
+ * large.  A record is stepped per code point over a W-word bit vector D of positions (bit 0: the virtual start, set before
+ * the first character only):
+ *     ctx = 1 << (prev_kind * 5 + kind(c))           kinds: 0 start / end, 1 '\n', 2 word, 3 Unicode-only word, 4 other
+ *     acc |= OR over accept groups a, not end-only:  (D & src_a) != 0 && (ctx_a & ctx)  ->  bit_a
+ *     D    = (((D << 1) & SHIFT) | (D & SELF) | OR over follow groups g: (D & src_g) != 0 && (ctx_g & ctx) -> dst_g) & B[class(c)]
+ * and at the end with next kind 0, every accept group counted.  Output bits are first_bit .. first_bit + n_patterns - 1 of the
+ * content verdict; a program's body DFA (class-indexed, not sticky, when there is one) owns the bits below first_bit.
+ * Every table is 16-byte aligned and the tables are contiguous from off_ascii (table_bytes): one bulk copy stages them. */
+typedef struct fei_prog_nfa {            /* 64 bytes */
+  uint32_t n_words;                      /* W: 1, 2, 4 or 8 32-bit words per position vector                               */
+  uint32_t n_pos;                        /* positions (bits) in use, the start bit included; <= 32 * W                      */
+  uint32_t n_classes, n_ranges, n_follow, n_accept, n_patterns, first_bit;
+  uint32_t off_ascii;                    /* uint16[128]: class | kind << 8 of each ASCII code point                         */
+  uint32_t off_range_lo;                 /* uint32[n_ranges]: first code point of each non-ASCII range, ascending, [0] = 0x80 */
+  uint32_t off_range_ck;                 /* uint16[n_ranges]: class | kind << 8 of each range                               */
+  uint32_t off_cls_b;                    /* uint32[n_classes][W]: B, the positions whose leaf holds the class                */
+  uint32_t off_masks;                    /* uint32[3][W]: SHIFT, SELF, START                                                 */
+  uint32_t off_follow;                   /* uint32[n_follow][2W + 1]: src[W], dst[W], ctx mask                               */
+  uint32_t off_accept;                   /* uint32[n_accept][W + 2]: src[W], ctx mask, output bit | end-only << 8             */
+  uint32_t table_bytes;                  /* from off_ascii to the end of the accept table                                     */
+} fei_prog_nfa;
+#define FEI_NFA_MAX_CLASSES 128
+#define FEI_NFA_MAX_RANGES  4096
+#define FEI_NFA_MAX_GROUPS  64           /* follow groups, and accept groups, each */
 
 typedef struct fei_prog_dfa {            /* 64 bytes; tables follow at the given offsets            */
   uint32_t n_states, n_cols;             /* n_cols == 256: byte-indexed rows; else class-indexed     */
