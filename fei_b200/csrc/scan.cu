@@ -12,7 +12,8 @@
 //          last value, a case-insensitive field lookup takes the first matching spelling) to the record's header lines:
 //          its header directory (hdir.cu: interned key + stripped value span per line; k_key_lut maps the corpus'
 //          distinct keys to the program's fields once per scan), or, for headers the directory cannot address, its
-//          text split / stripped like utils.py:113-118.  Every string condition is an output bit of a byte DFA; the program
+//          text split / stripped like utils.py:113-118.  Every string condition is an output bit of a byte DFA (or of the field's
+//          position automaton, head_nfa_run, for patterns the DFA refuses; k_head_meta<kFused, true> / k_head_parse<true>); the program
 //          head (conditions + small automata) is staged into shared memory by a TMA bulk copy per CTA.
 //          Writes alive[i] = bitmask of queries whose non-content conditions all hold.
 // k_body : one warp per group of 32 records in the warp-transposed body tiles (corpus.h): each
@@ -119,6 +120,130 @@ template <class Run> __device__ __forceinline__ uint32_t dfa_run_at(const uint8_
 }
 __device__ __forceinline__ uint32_t dfa_run_at(const uint8_t* blob, uint32_t off, bool in_smem, const uint8_t* p, uint32_t len) {
   return dfa_run_at(blob, off, in_smem, [&](auto d) { return d.span(p, len); });
+}
+
+// ---------------------------------------------------------------- position automaton step (content and head fields)
+// One code point of a fei_prog_nfa (feiscan_prog.h) over a W-word bit vector of NFA positions:
+//     D' = (((D << 1) & SHIFT) | (D & SELF) | OR_g [(D & src_g) && ctx ok] dst_g) & B[class]
+// The tables are read through generic pointers: k_body_nfa's staged shared-memory copy, or a head field's section in the staged
+// program head or in the global program.
+struct NfaTables {
+  const uint16_t* ascii; const uint32_t* range_lo; const uint16_t* range_ck; const uint32_t* cls_b;
+  const uint32_t* masks; const uint32_t* follow; const uint32_t* accept;
+  uint32_t n_ranges, n_follow, n_accept;
+  // the tables of section nd, whose bytes [off_ascii, off_ascii + table_bytes) start at tab
+  __device__ __forceinline__ NfaTables(const fei_prog_nfa* nd, const uint8_t* tab) {
+    ascii = reinterpret_cast<const uint16_t*>(tab);
+    range_lo = reinterpret_cast<const uint32_t*>(tab + (nd->off_range_lo - nd->off_ascii));
+    range_ck = reinterpret_cast<const uint16_t*>(tab + (nd->off_range_ck - nd->off_ascii));
+    cls_b = reinterpret_cast<const uint32_t*>(tab + (nd->off_cls_b - nd->off_ascii));
+    masks = reinterpret_cast<const uint32_t*>(tab + (nd->off_masks - nd->off_ascii));
+    follow = reinterpret_cast<const uint32_t*>(tab + (nd->off_follow - nd->off_ascii));
+    accept = reinterpret_cast<const uint32_t*>(tab + (nd->off_accept - nd->off_ascii));
+    n_ranges = nd->n_ranges; n_follow = nd->n_follow; n_accept = nd->n_accept;
+  }
+  __device__ __forceinline__ uint32_t class_kind(uint32_t cp) const {     // class | kind << 8
+    if (cp < 0x80u) return ascii[cp];
+    uint32_t lo = 0, hi = n_ranges - 1;
+    while (lo < hi) {
+      const uint32_t mid = (lo + hi + 1) >> 1;
+      if (range_lo[mid] <= cp) lo = mid; else hi = mid - 1;
+    }
+    return range_ck[lo];
+  }
+};
+
+template <int W>
+struct Nfa {
+  uint32_t d[W];                     // active positions
+  uint32_t prev;                     // context kind of the last code point (0: none yet)
+  uint32_t cp, need;                 // UTF-8 decoder: code point so far, continuation bytes still to come
+  uint32_t acc;                      // output bits of the accepts met so far (end-only accepts not included)
+  __device__ __forceinline__ void reset(const NfaTables& t) {
+#pragma unroll
+    for (int k = 0; k < W; ++k) d[k] = t.masks[2 * W + k];
+    prev = 0; cp = 0; need = 0; acc = 0;
+  }
+  __device__ __forceinline__ bool any(const uint32_t* src) const {
+    uint32_t x = 0;
+#pragma unroll
+    for (int k = 0; k < W; ++k) x |= d[k] & src[k];
+    return x != 0;
+  }
+  __device__ __forceinline__ uint32_t accepts(const NfaTables& t, uint32_t ctx, bool at_end) const {
+    uint32_t m = 0;
+    for (uint32_t g = 0; g < t.n_accept; ++g) {
+      const uint32_t* r = t.accept + g * (W + 2);
+      const uint32_t info = r[W + 1];
+      if ((r[W] & ctx) && (at_end || !(info >> 8)) && any(r)) m |= 1u << (info & 31u);
+    }
+    return m;
+  }
+  __device__ __forceinline__ void step_cp(const NfaTables& t, uint32_t c) {
+    const uint32_t ck = t.class_kind(c);
+    const uint32_t kind = ck >> 8;
+    const uint32_t ctx = 1u << (prev * 5u + kind);
+    acc |= accepts(t, ctx, false);
+    uint32_t n[W];
+#pragma unroll
+    for (int k = 0; k < W; ++k) {
+      const uint32_t sh = k ? __funnelshift_l(d[k - 1], d[k], 1) : d[0] << 1;
+      n[k] = (sh & t.masks[k]) | (d[k] & t.masks[W + k]);
+    }
+    for (uint32_t g = 0; g < t.n_follow; ++g) {
+      const uint32_t* r = t.follow + g * (2 * W + 1);
+      if ((r[2 * W] & ctx) && any(r)) {
+#pragma unroll
+        for (int k = 0; k < W; ++k) n[k] |= r[W + k];
+      }
+    }
+    const uint32_t* b = t.cls_b + (ck & 0xFFu) * W;
+#pragma unroll
+    for (int k = 0; k < W; ++k) d[k] = n[k] & b[k];
+    prev = kind;
+  }
+  // one byte of UTF-8 text
+  __device__ __forceinline__ void byte(const NfaTables& t, uint32_t b) {
+    if (b < 0x80u) { step_cp(t, b); return; }                        // ASCII: one byte, one code point
+    if (b >= 0xC0u) { need = b >= 0xF0u ? 3u : b >= 0xE0u ? 2u : 1u; cp = b & (0x3Fu >> need); return; }
+    cp = (cp << 6) | (b & 0x3Fu);
+    if (--need == 0) step_cp(t, cp);
+  }
+  __device__ __forceinline__ uint32_t finish(const NfaTables& t) const { return acc | accepts(t, 1u << (prev * 5u), true); }
+};
+
+// A head field's position automaton (the section at `off` of the program at `prog`, staged or global) over one value of len
+// bytes: byte j at p[(j >> 4) * stride + (j & 15)] -- a span of header text or a formatted buffer with stride 16, value-column
+// units (Dfa::units) with the plane stride -- or, with p == nullptr, byte j of `reg` (flags8).  Out of line: the head kernels'
+// DFA paths do not pay its registers, and one copy serves every caller.
+template <int W>
+__device__ __forceinline__ uint32_t nfa_run(const NfaTables& t, const uint8_t* p, uint64_t stride, uint32_t len, unsigned long long reg) {
+  Nfa<W> nfa;
+  nfa.reset(t);
+  for (uint32_t j = 0; j < len; ++j) nfa.byte(t, p ? p[(j >> 4) * stride + (j & 15u)] : (uint32_t)(reg >> (8 * j)) & 0xFFu);
+  return nfa.finish(t);
+}
+__device__ __noinline__ uint32_t head_nfa_run(const uint8_t* prog, uint32_t off, const uint8_t* p, uint64_t stride, uint32_t len,
+                                              unsigned long long reg) {
+  const fei_prog_nfa* nd = reinterpret_cast<const fei_prog_nfa*>(prog + off);
+  const NfaTables t(nd, prog + nd->off_ascii);
+  switch (nd->n_words) {                                               // check_prog: 1, 2, 4 or 8
+    case 1: return nfa_run<1>(t, p, stride, len, reg);
+    case 2: return nfa_run<2>(t, p, stride, len, reg);
+    case 4: return nfa_run<4>(t, p, stride, len, reg);
+    default: return nfa_run<8>(t, p, stride, len, reg);
+  }
+}
+// A head field's verdict over one value: its DFA's bits, run(dfa), and its position automaton's over the same bytes (either
+// part may be absent).  Only kHeadNfa instances call it; the others run the DFA alone, as before there were head automata.
+template <class Run>
+__device__ __forceinline__ uint32_t field_run(const uint8_t* prog, bool in_smem, uint32_t off_dfa, uint32_t off_nfa, Run run,
+                                              const uint8_t* p, uint64_t stride, uint32_t len) {
+  return (off_dfa ? dfa_run_at(prog, off_dfa, in_smem, run) : 0u) | (off_nfa ? head_nfa_run(prog, off_nfa, p, stride, len, 0) : 0u);
+}
+// fei_prog_head_nfa entry k (0 flags, 1 + name field)
+__device__ __forceinline__ uint32_t head_nfa_off(const uint8_t* prog, const fei_prog_hdr* ph, int k) {
+  return ph->off_head_nfa ? reinterpret_cast<const uint32_t*>(prog + ph->off_head_nfa)[k] : 0u;
 }
 
 // ---------------------------------------------------------------- header field lookup
@@ -289,20 +414,40 @@ __device__ __forceinline__ uint32_t format_datetime(int64_t wall, uint8_t* out) 
 // HeadArgs, like a dynamic index into one of its arrays, makes ptxas copy the whole struct to local memory -- that, via the aux
 // column array, more than doubled the time of the cfg2 head pass.)
 struct NameArgs { const uint8_t* prog; const uint8_t* name; const uint64_t* name_off; const uint16_t* name_spans; const int64_t* ts; const int64_t* wall; bool prog_in_smem; };
+template <bool kHeadNfa>
 __device__ __noinline__ void eval_name_fields(const NameArgs a, const fei_prog_hdr* ph, uint64_t rec, uint32_t* name_acc) {
-  for (int k = 0; k < 3; ++k) {
-    if (!ph->off_name_dfa[k]) continue;
-    const uint8_t* nb = a.name + a.name_off[rec];
-    uint32_t nl = (uint32_t)(a.name_off[rec + 1] - a.name_off[rec]);
-    if (k > 0) { const uint16_t* sp = a.name_spans + 4 * rec + 2 * (k - 1); nb += sp[0]; nl = sp[1]; }
-    name_acc[k] = dfa_run_at(a.prog, ph->off_name_dfa[k], a.prog_in_smem, nb, nl);
+  if constexpr (!kHeadNfa) {
+    for (int k = 0; k < 3; ++k) {
+      if (!ph->off_name_dfa[k]) continue;
+      const uint8_t* nb = a.name + a.name_off[rec];
+      uint32_t nl = (uint32_t)(a.name_off[rec + 1] - a.name_off[rec]);
+      if (k > 0) { const uint16_t* sp = a.name_spans + 4 * rec + 2 * (k - 1); nb += sp[0]; nl = sp[1]; }
+      name_acc[k] = dfa_run_at(a.prog, ph->off_name_dfa[k], a.prog_in_smem, nb, nl);
+    }
+    // str(timestamp) and str(datetime.fromtimestamp(ts))
+    if (ph->off_meta_dfa[0]) { uint8_t buf[24]; const uint32_t nl = format_u64(a.ts[rec] < 0 ? 0ull : (unsigned long long)a.ts[rec], buf); name_acc[3] = dfa_run_at(a.prog, ph->off_meta_dfa[0], a.prog_in_smem, buf, nl); }
+    if (ph->off_meta_dfa[1]) { uint8_t buf[24]; const uint32_t nl = format_datetime(a.wall[rec], buf); name_acc[4] = dfa_run_at(a.prog, ph->off_meta_dfa[1], a.prog_in_smem, buf, nl); }
+  } else {                                                     // the same fields, each through its DFA and / or position automaton
+    for (int k = 0; k < FEI_NAME_FIELDS; ++k) {
+      const uint32_t off_dfa = k < 3 ? ph->off_name_dfa[k] : ph->off_meta_dfa[k - 3], off_nfa = head_nfa_off(a.prog, ph, 1 + k);
+      if (!off_dfa && !off_nfa) continue;
+      uint8_t buf[24];
+      const uint8_t* nb = buf;
+      uint32_t nl;
+      if (k == 3) nl = format_u64(a.ts[rec] < 0 ? 0ull : (unsigned long long)a.ts[rec], buf);
+      else if (k == 4) nl = format_datetime(a.wall[rec], buf);
+      else {
+        nb = a.name + a.name_off[rec]; nl = (uint32_t)(a.name_off[rec + 1] - a.name_off[rec]);
+        if (k > 0) { const uint16_t* sp = a.name_spans + 4 * rec + 2 * (k - 1); nb += sp[0]; nl = sp[1]; }
+      }
+      name_acc[k] = field_run(a.prog, a.prog_in_smem, off_dfa, off_nfa, [&](auto d) { return d.span(nb, nl); }, nb, 16, nl);
+    }
   }
-  // str(timestamp) and str(datetime.fromtimestamp(ts))
-  if (ph->off_meta_dfa[0]) { uint8_t buf[24]; const uint32_t nl = format_u64(a.ts[rec] < 0 ? 0ull : (unsigned long long)a.ts[rec], buf); name_acc[3] = dfa_run_at(a.prog, ph->off_meta_dfa[0], a.prog_in_smem, buf, nl); }
-  if (ph->off_meta_dfa[1]) { uint8_t buf[24]; const uint32_t nl = format_datetime(a.wall[rec], buf); name_acc[4] = dfa_run_at(a.prog, ph->off_meta_dfa[1], a.prog_in_smem, buf, nl); }
 }
 
-// Phase 2 for one record: header fields (if `parse`), name fields, evaluation of the queries left in `pre`.
+// Phase 2 for one record: header fields (if `parse`), name fields, evaluation of the queries left in `pre`.  kHeadNfa: the
+// program has head position automata (a slot may then have no DFA).
+template <bool kHeadNfa>
 __device__ void head_finish(const HeadArgs& a, uint64_t rec, uint32_t pre, uint32_t flags_acc, bool parse) {
   const fei_prog_hdr* ph = reinterpret_cast<const fei_prog_hdr*>(a.prog);
   const fei_prog_cond* conds = reinterpret_cast<const fei_prog_cond*>(a.prog + ph->off_conds);
@@ -323,7 +468,10 @@ __device__ void head_finish(const HeadArgs& a, uint64_t rec, uint32_t pre, uint3
       if (len == kColAbsent) continue;
       if (len == kColWalk) { walk = true; break; }
       const uint8_t* unit = a.col_planes + (uint64_t)col * kColUnits * a.n * 16 + rec * 16;
-      slot_acc[s] = dfa_run_at(a.prog, slots[s].off_val_dfa, a.prog_in_smem, [&](auto d) { return d.units(unit, a.n * 16, len); });
+      if constexpr (kHeadNfa)
+        slot_acc[s] = field_run(a.prog, a.prog_in_smem, slots[s].off_val_dfa, slots[s].off_val_nfa, [&](auto d) { return d.units(unit, a.n * 16, len); },
+                                unit, a.n * 16, len);
+      else slot_acc[s] = dfa_run_at(a.prog, slots[s].off_val_dfa, a.prog_in_smem, [&](auto d) { return d.units(unit, a.n * 16, len); });
       present |= 1u << s;
     }
     if (walk) {
@@ -334,7 +482,10 @@ __device__ void head_finish(const HeadArgs& a, uint64_t rec, uint32_t pre, uint3
       uint32_t val_off[FEI_MAX_SLOTS], val_len[FEI_MAX_SLOTS];
       uint32_t any_mask = 0;                                   // mode-2 slots ("any header value", utils.py:333-336) already accumulated
       auto any = [&](int s, uint32_t off, uint32_t len) {
-        const uint32_t acc = dfa_run_at(a.prog, slots[s].off_val_dfa, a.prog_in_smem, h + off, len);
+        uint32_t acc;
+        if constexpr (kHeadNfa)
+          acc = field_run(a.prog, a.prog_in_smem, slots[s].off_val_dfa, slots[s].off_val_nfa, [&](auto d) { return d.span(h + off, len); }, h + off, 16, len);
+        else acc = dfa_run_at(a.prog, slots[s].off_val_dfa, a.prog_in_smem, h + off, len);
         slot_acc[s] = (any_mask >> s & 1u) ? (slot_acc[s] | acc) : acc;
         any_mask |= 1u << s;
       };
@@ -344,18 +495,23 @@ __device__ void head_finish(const HeadArgs& a, uint64_t rec, uint32_t pre, uint3
           : header_lookup<FEI_MAX_SLOTS>(DirLines{ent, n_ent, a.key_lut}, mode, val_off, val_len, any);
       for (uint32_t m = present; m; m &= m - 1) {
         const int s = __ffs(m) - 1;
-        slot_acc[s] = dfa_run_at(a.prog, slots[s].off_val_dfa, a.prog_in_smem, h + val_off[s], val_len[s]);
+        const uint8_t* v = h + val_off[s];
+        if constexpr (kHeadNfa)
+          slot_acc[s] = field_run(a.prog, a.prog_in_smem, slots[s].off_val_dfa, slots[s].off_val_nfa, [&](auto d) { return d.span(v, val_len[s]); }, v, 16, val_len[s]);
+        else slot_acc[s] = dfa_run_at(a.prog, slots[s].off_val_dfa, a.prog_in_smem, h + val_off[s], val_len[s]);
       }
       present |= any_mask;
     }
   }
   for (uint32_t s = 0; s < nslots; ++s)
     if (!(present >> s & 1) && slots[s].empty_if_missing) {   // headers.get("Status", "")
-      slot_acc[s] = reinterpret_cast<const fei_prog_dfa*>(a.prog + slots[s].off_val_dfa)->empty_acc;
+      if constexpr (!kHeadNfa) slot_acc[s] = reinterpret_cast<const fei_prog_dfa*>(a.prog + slots[s].off_val_dfa)->empty_acc;
+      else slot_acc[s] = (slots[s].off_val_dfa ? reinterpret_cast<const fei_prog_dfa*>(a.prog + slots[s].off_val_dfa)->empty_acc : 0u) |
+                         (slots[s].off_val_nfa ? head_nfa_run(a.prog, slots[s].off_val_nfa, nullptr, 0, 0, 0) : 0u);
       present |= 1u << s;
     }
   uint32_t name_acc[FEI_NAME_FIELDS] = {0, 0, 0, 0, 0};
-  if (pre & ph->name_mask) eval_name_fields(NameArgs{a.prog, a.name, a.name_off, a.name_spans, a.ts, a.wall, (bool)a.prog_in_smem}, ph, rec, name_acc);
+  if (pre & ph->name_mask) eval_name_fields<kHeadNfa>(NameArgs{a.prog, a.name, a.name_off, a.name_spans, a.ts, a.wall, (bool)a.prog_in_smem}, ph, rec, name_acc);
   uint32_t alive = 0;
   for (uint32_t q = 0; q < ph->n_queries; ++q) {
     if (!(pre >> q & 1)) continue;
@@ -429,7 +585,7 @@ struct Survivor { uint32_t rec, pre, flags_acc; };
 
 constexpr int kMetaPer = 4;     // records per thread: the (uniform) condition fetch / decode is paid once for four records
 
-template <bool kFused>
+template <bool kFused, bool kHeadNfa>
 __global__ void __launch_bounds__(256, 5) k_head_meta(HeadArgs a, Survivor* __restrict__ list, unsigned int* __restrict__ count) {
   __shared__ __align__(128) uint8_t sprog[kHeadProgSmem];
   __shared__ uint64_t bar;
@@ -455,6 +611,11 @@ __global__ void __launch_bounds__(256, 5) k_head_meta(HeadArgs a, Survivor* __re
     for (int r = 0; r < kMetaPer; ++r)
       flags_acc[r] = dfa_run_at(a.prog, ph->off_flags_dfa, a.prog_in_smem, [&](auto d) { return d.u64(f8[r], (uint32_t)(f8[r] >> 56)); });
   }
+  if constexpr (kHeadNfa) {
+    if (const uint32_t off = head_nfa_off(a.prog, ph, 0)) {
+      for (int r = 0; r < kMetaPer; ++r) flags_acc[r] |= head_nfa_run(a.prog, off, nullptr, 0, (uint32_t)(f8[r] >> 56), f8[r]);
+    }
+  }
   for (uint32_t q = 0; q < ph->n_queries; ++q) {
     bool ok[kMetaPer];
 #pragma unroll
@@ -476,7 +637,7 @@ __global__ void __launch_bounds__(256, 5) k_head_meta(HeadArgs a, Survivor* __re
       const uint64_t i = base + (uint64_t)r * 256;
       if (!valid[r]) continue;
       if ((pre[r] & later_mask) == 0) a.alive[i] = pre[r];
-      else head_finish(a, i, pre[r], flags_acc[r], (pre[r] & ph->slot_mask) != 0);
+      else head_finish<kHeadNfa>(a, i, pre[r], flags_acc[r], (pre[r] & ph->slot_mask) != 0);
     }
     return;
   }
@@ -511,6 +672,7 @@ __global__ void __launch_bounds__(256, 5) k_head_meta(HeadArgs a, Survivor* __re
   }
 }
 
+template <bool kHeadNfa>
 __global__ void __launch_bounds__(256, 5) k_head_parse(HeadArgs a, const Survivor* __restrict__ list, const unsigned int* __restrict__ n_list) {
   __shared__ __align__(128) uint8_t sprog[kHeadProgSmem];
   __shared__ uint64_t bar;
@@ -522,7 +684,7 @@ __global__ void __launch_bounds__(256, 5) k_head_parse(HeadArgs a, const Survivo
   if (t >= n_surv) return;
   const fei_prog_hdr* ph = reinterpret_cast<const fei_prog_hdr*>(a.prog);
   const Survivor sv = list[t];
-  head_finish(a, sv.rec, sv.pre, sv.flags_acc, (sv.pre & ph->slot_mask) != 0);
+  head_finish<kHeadNfa>(a, sv.rec, sv.pre, sv.flags_acc, (sv.pre & ph->slot_mask) != 0);
 }
 
 // ---------------------------------------------------------------- body kernel
@@ -1423,81 +1585,6 @@ __global__ void __launch_bounds__(kBodyThreads, 1) k_body_gather(BodyArgs a, con
 // after the scan and the multi-GPU hook copies the masks (no window work in the kernel).
 template <int W> struct NfaThreads { static constexpr int value = W <= 4 ? 1024 : 512; };
 
-struct NfaTables {                   // shared-memory views of a staged fei_prog_nfa
-  const uint16_t* ascii; const uint32_t* range_lo; const uint16_t* range_ck; const uint32_t* cls_b;
-  const uint32_t* masks; const uint32_t* follow; const uint32_t* accept;
-  uint32_t n_ranges, n_follow, n_accept;
-  __device__ __forceinline__ uint32_t class_kind(uint32_t cp) const {     // class | kind << 8
-    if (cp < 0x80u) return ascii[cp];
-    uint32_t lo = 0, hi = n_ranges - 1;
-    while (lo < hi) {
-      const uint32_t mid = (lo + hi + 1) >> 1;
-      if (range_lo[mid] <= cp) lo = mid; else hi = mid - 1;
-    }
-    return range_ck[lo];
-  }
-};
-
-template <int W>
-struct BodyNfa {
-  uint32_t d[W];                     // active positions
-  uint32_t prev;                     // context kind of the last code point (0: none yet)
-  uint32_t cp, need;                 // UTF-8 decoder: code point so far, continuation bytes still to come
-  uint32_t acc;                      // output bits of the accepts met so far (end-only accepts not included)
-  __device__ __forceinline__ void reset(const NfaTables& t) {
-#pragma unroll
-    for (int k = 0; k < W; ++k) d[k] = t.masks[2 * W + k];
-    prev = 0; cp = 0; need = 0; acc = 0;
-  }
-  __device__ __forceinline__ bool any(const uint32_t* src) const {
-    uint32_t x = 0;
-#pragma unroll
-    for (int k = 0; k < W; ++k) x |= d[k] & src[k];
-    return x != 0;
-  }
-  __device__ __forceinline__ uint32_t accepts(const NfaTables& t, uint32_t ctx, bool at_end) const {
-    uint32_t m = 0;
-    for (uint32_t g = 0; g < t.n_accept; ++g) {
-      const uint32_t* r = t.accept + g * (W + 2);
-      const uint32_t info = r[W + 1];
-      if ((r[W] & ctx) && (at_end || !(info >> 8)) && any(r)) m |= 1u << (info & 31u);
-    }
-    return m;
-  }
-  __device__ __forceinline__ void step_cp(const NfaTables& t, uint32_t c) {
-    const uint32_t ck = t.class_kind(c);
-    const uint32_t kind = ck >> 8;
-    const uint32_t ctx = 1u << (prev * 5u + kind);
-    acc |= accepts(t, ctx, false);
-    uint32_t n[W];
-#pragma unroll
-    for (int k = 0; k < W; ++k) {
-      const uint32_t sh = k ? __funnelshift_l(d[k - 1], d[k], 1) : d[0] << 1;
-      n[k] = (sh & t.masks[k]) | (d[k] & t.masks[W + k]);
-    }
-    for (uint32_t g = 0; g < t.n_follow; ++g) {
-      const uint32_t* r = t.follow + g * (2 * W + 1);
-      if ((r[2 * W] & ctx) && any(r)) {
-#pragma unroll
-        for (int k = 0; k < W; ++k) n[k] |= r[W + k];
-      }
-    }
-    const uint32_t* b = t.cls_b + (ck & 0xFFu) * W;
-#pragma unroll
-    for (int k = 0; k < W; ++k) d[k] = n[k] & b[k];
-    prev = kind;
-  }
-  // one stored tile byte
-  __device__ __forceinline__ void byte(const NfaTables& t, uint32_t stored) {
-    const uint32_t b = tile_byte_unperm((uint8_t)stored);
-    if (b < 0x80u) { step_cp(t, b); return; }                        // ASCII: one byte, one code point
-    if (b >= 0xC0u) { need = b >= 0xF0u ? 3u : b >= 0xE0u ? 2u : 1u; cp = b & (0x3Fu >> need); return; }
-    cp = (cp << 6) | (b & 0x3Fu);
-    if (--need == 0) step_cp(t, cp);
-  }
-  __device__ __forceinline__ uint32_t finish(const NfaTables& t) const { return acc | accepts(t, 1u << (prev * 5u), true); }
-};
-
 // Stage the body DFA's tables (bytes0, may be 0) and the position automaton's behind them with one mbarrier.
 __device__ __forceinline__ void stage_two_tables(uint8_t* dst0, const uint8_t* src0, uint32_t bytes0, uint8_t* dst1, const uint8_t* src1,
                                                  uint32_t bytes1, uint64_t* bar) {
@@ -1534,15 +1621,7 @@ __global__ void __launch_bounds__(NfaThreads<W>::value, 1) k_body_nfa(BodyArgs a
   const uint32_t dfa_bytes = kHasDfa ? dd->table_bytes : 0u;
   uint8_t* nsm = smem + dfa_bytes;                 // both table sizes are multiples of 16
   stage_two_tables(smem, kHasDfa ? a.prog + dd->off_trans : nullptr, dfa_bytes, nsm, a.prog + nd->off_ascii, nd->table_bytes, &bar);
-  NfaTables t;
-  t.ascii = reinterpret_cast<const uint16_t*>(nsm);
-  t.range_lo = reinterpret_cast<const uint32_t*>(nsm + (nd->off_range_lo - nd->off_ascii));
-  t.range_ck = reinterpret_cast<const uint16_t*>(nsm + (nd->off_range_ck - nd->off_ascii));
-  t.cls_b = reinterpret_cast<const uint32_t*>(nsm + (nd->off_cls_b - nd->off_ascii));
-  t.masks = reinterpret_cast<const uint32_t*>(nsm + (nd->off_masks - nd->off_ascii));
-  t.follow = reinterpret_cast<const uint32_t*>(nsm + (nd->off_follow - nd->off_ascii));
-  t.accept = reinterpret_cast<const uint32_t*>(nsm + (nd->off_accept - nd->off_ascii));
-  t.n_ranges = nd->n_ranges; t.n_follow = nd->n_follow; t.n_accept = nd->n_accept;
+  const NfaTables t(nd, nsm);
   BodyDfa<false, 0> d;
   const uint32_t* endout = nullptr;
   uint32_t dfa_start = 0;
@@ -1554,7 +1633,7 @@ __global__ void __launch_bounds__(NfaThreads<W>::value, 1) k_body_nfa(BodyArgs a
     endout = reinterpret_cast<const uint32_t*>(smem + (dd->off_endout - dd->off_trans));
     dfa_start = dd->start;
   }
-  BodyNfa<W> nfa;
+  Nfa<W> nfa;
   const uint32_t all_q = nq >= 32 ? 0xFFFFFFFFu : ((1u << nq) - 1u);
   const int lane = threadIdx.x & 31;
   unsigned long long touched = 0;
@@ -1606,7 +1685,7 @@ __global__ void __launch_bounds__(NfaThreads<W>::value, 1) k_body_nfa(BodyArgs a
           const uint32_t b = v.x & 0xFFu;
           v.x = __funnelshift_r(v.x, v.y, 8); v.y = __funnelshift_r(v.y, v.z, 8); v.z = __funnelshift_r(v.z, v.w, 8); v.w >>= 8;
           if constexpr (kHasDfa) d.step(b);
-          nfa.byte(t, b);
+          nfa.byte(t, tile_byte_unperm((uint8_t)b));
         }
       }
       cur = nxt; row = next_row;
@@ -1784,11 +1863,11 @@ __global__ void __launch_bounds__(256) k_list_checksum(const T* __restrict__ v, 
 static int check_prog(const uint8_t* prog, uint64_t len) {
   if (!prog || len < sizeof(fei_prog_hdr)) { set_error("program blob too small"); return FEI_E_BADARG; }
   fei_prog_hdr h; memcpy(&h, prog, sizeof(h));
-  if (h.magic != FEI_PROG_MAGIC || (h.version != FEI_PROG_VERSION && h.version != FEI_PROG_VERSION_NFA) ||
-      (h.version == FEI_PROG_VERSION_NFA) != (h.off_body_nfa != 0)) { set_error("bad program magic/version"); return FEI_E_BADARG; }
+  if (h.magic != FEI_PROG_MAGIC || (h.version != FEI_PROG_VERSION && h.version != FEI_PROG_VERSION_NFA)) { set_error("bad program magic/version"); return FEI_E_BADARG; }
   if (h.total_bytes != len) { set_error("program length mismatch (%u vs %llu)", h.total_bytes, (unsigned long long)len); return FEI_E_BADARG; }
   if (h.n_queries == 0 || h.n_queries > FEI_MAX_QUERIES) { set_error("1..32 queries per program"); return FEI_E_BADARG; }
   if (h.n_slots > FEI_MAX_SLOTS) { set_error("at most %d header slots per program", FEI_MAX_SLOTS); return FEI_E_UNSUPPORTED; }
+  if (h.head_bytes > h.total_bytes || (h.head_bytes & 15u)) { set_error("bad head_bytes in program"); return FEI_E_BADARG; }
   auto in = [&](uint64_t off, uint64_t sz) { return off % 16 == 0 && off + sz <= len; };
   if (!in(h.off_conds, (uint64_t)h.n_conds * sizeof(fei_prog_cond)) || !in(h.off_queries, (uint64_t)h.n_queries * sizeof(fei_prog_query)) ||
       !in(h.off_slots, (uint64_t)h.n_slots * sizeof(fei_prog_slot))) { set_error("program section out of bounds"); return FEI_E_BADARG; }
@@ -1804,20 +1883,23 @@ static int check_prog(const uint8_t* prog, uint64_t len) {
   };
   if (!dfa_ok(h.off_key_dfa) || !dfa_ok(h.off_body_dfa) || !dfa_ok(h.off_flags_dfa) || !dfa_ok(h.off_name_dfa[0]) ||
       !dfa_ok(h.off_name_dfa[1]) || !dfa_ok(h.off_name_dfa[2]) || !dfa_ok(h.off_meta_dfa[0]) || !dfa_ok(h.off_meta_dfa[1])) { set_error("bad DFA descriptor in program"); return FEI_E_BADARG; }
-  const fei_prog_slot* sl = reinterpret_cast<const fei_prog_slot*>(prog + h.off_slots);
-  for (uint32_t s = 0; s < h.n_slots; ++s) if (!sl[s].off_val_dfa || !dfa_ok(sl[s].off_val_dfa)) { set_error("bad slot DFA"); return FEI_E_BADARG; }
-  if (h.n_slots && !h.off_key_dfa) { set_error("slots without a key DFA"); return FEI_E_BADARG; }
-  if (h.off_body_nfa) {                            // the content position automaton: every table inside its table_bytes
-    if (!in(h.off_body_nfa, sizeof(fei_prog_nfa))) { set_error("content position automaton out of bounds"); return FEI_E_BADARG; }
-    fei_prog_nfa a; memcpy(&a, prog + h.off_body_nfa, sizeof(a));
+  // A position automaton section (0 = none): every table inside its table_bytes; a head one inside [0, head_bytes) when the head
+  // kernels stage the head.
+  uint32_t n_nfa = 0;
+  auto nfa_ok = [&](uint32_t off, bool head) {
+    if (!off) return true;
+    ++n_nfa;
+    if (!in(off, sizeof(fei_prog_nfa))) return false;
+    fei_prog_nfa a; memcpy(&a, prog + off, sizeof(a));
     const uint64_t W = a.n_words, end = (uint64_t)a.off_ascii + a.table_bytes;
-    auto tab = [&](uint64_t off, uint64_t sz) { return off % 16 == 0 && off >= a.off_ascii && off + sz <= end; };
+    auto tab = [&](uint64_t o, uint64_t sz) { return o % 16 == 0 && o >= a.off_ascii && o + sz <= end; };
     bool ok = (W == 1 || W == 2 || W == 4 || W == 8) && a.n_pos >= 1 && a.n_pos <= 32 * W && a.n_classes >= 1 &&
               a.n_classes <= FEI_NFA_MAX_CLASSES && a.n_ranges >= 1 && a.n_ranges <= FEI_NFA_MAX_RANGES &&
               a.n_follow <= FEI_NFA_MAX_GROUPS && a.n_accept <= FEI_NFA_MAX_GROUPS && a.first_bit + (uint64_t)a.n_patterns <= 32 &&
               a.table_bytes % 16 == 0 && in(a.off_ascii, a.table_bytes) && tab(a.off_ascii, 2 * 128) &&
               tab(a.off_range_lo, 4ull * a.n_ranges) && tab(a.off_range_ck, 2ull * a.n_ranges) && tab(a.off_cls_b, 4ull * W * a.n_classes) &&
-              tab(a.off_masks, 12ull * W) && tab(a.off_follow, 4ull * (2 * W + 1) * a.n_follow) && tab(a.off_accept, 4ull * (W + 2) * a.n_accept);
+              tab(a.off_masks, 12ull * W) && tab(a.off_follow, 4ull * (2 * W + 1) * a.n_follow) && tab(a.off_accept, 4ull * (W + 2) * a.n_accept) &&
+              (!head || !h.head_bytes || (off + sizeof(fei_prog_nfa) <= h.head_bytes && end <= h.head_bytes));
     if (ok) {                                      // class ids index cls_b, kinds are 0..4, the range table starts at 0x80
       const uint16_t* asc = reinterpret_cast<const uint16_t*>(prog + a.off_ascii);
       const uint16_t* rck = reinterpret_cast<const uint16_t*>(prog + a.off_range_ck);
@@ -1828,12 +1910,27 @@ static int check_prog(const uint8_t* prog, uint64_t len) {
       const uint32_t* acc = reinterpret_cast<const uint32_t*>(prog + a.off_accept);
       for (uint32_t g = 0; g < a.n_accept && ok; ++g) ok = (acc[g * (W + 2) + W + 1] & 0xFFu) < 32;
     }
-    if (!ok) { set_error("bad content position automaton in program"); return FEI_E_BADARG; }
+    return ok;
+  };
+  const fei_prog_slot* sl = reinterpret_cast<const fei_prog_slot*>(prog + h.off_slots);
+  for (uint32_t s = 0; s < h.n_slots; ++s)
+    if ((!sl[s].off_val_dfa && !sl[s].off_val_nfa) || !dfa_ok(sl[s].off_val_dfa) || !nfa_ok(sl[s].off_val_nfa, true)) { set_error("bad slot automaton"); return FEI_E_BADARG; }
+  if (h.n_slots && !h.off_key_dfa) { set_error("slots without a key DFA"); return FEI_E_BADARG; }
+  if (h.off_head_nfa) {                            // flags and name fields
+    fei_prog_head_nfa hn;
+    if (!in(h.off_head_nfa, sizeof(hn)) || (h.head_bytes && h.off_head_nfa + sizeof(hn) > h.head_bytes)) { set_error("head position automata out of bounds"); return FEI_E_BADARG; }
+    memcpy(&hn, prog + h.off_head_nfa, sizeof(hn));
+    bool ok = nfa_ok(hn.off_flags_nfa, true);
+    for (int k = 0; k < FEI_NAME_FIELDS && ok; ++k) ok = nfa_ok(hn.off_name_nfa[k], true);
+    if (!ok) { set_error("bad flags / name position automaton in program"); return FEI_E_BADARG; }
+  }
+  if (!nfa_ok(h.off_body_nfa, false)) { set_error("bad content position automaton in program"); return FEI_E_BADARG; }
+  if ((h.version == FEI_PROG_VERSION_NFA) != (n_nfa != 0)) { set_error("bad program magic/version"); return FEI_E_BADARG; }
+  if (h.off_body_nfa) {
     fei_prog_dfa d{};
     if (h.off_body_dfa) memcpy(&d, prog + h.off_body_dfa, sizeof(d));
     if (h.off_body_dfa && (d.n_cols == 256 || d.sticky || d.table_bytes % 16)) { set_error("the body DFA next to a position automaton must be class-indexed"); return FEI_E_BADARG; }
   }
-  if (h.head_bytes > h.total_bytes || (h.head_bytes & 15u)) { set_error("bad head_bytes in program"); return FEI_E_BADARG; }
   const fei_prog_query* qs = reinterpret_cast<const fei_prog_query*>(prog + h.off_queries);
   for (uint32_t q = 0; q < h.n_queries; ++q) if (qs[q].cond_begin > qs[q].cond_end || qs[q].cond_end > h.n_conds) { set_error("bad query range"); return FEI_E_BADARG; }
   return FEI_OK;
@@ -1864,7 +1961,12 @@ int run_scan(fei_corpus* c, const uint8_t* prog, uint64_t prog_len, int compact_
   bool need_head = h.head_mask != 0;
   bool need_body = (h.off_body_dfa != 0 || h.off_body_nfa != 0) && h.body_mask != 0;
   const bool nfa = need_body && h.off_body_nfa != 0;           // k_body_nfa (with the body DFA, if any, stepped alongside)
-  if ((h.off_name_dfa[0] || h.off_name_dfa[1] || h.off_name_dfa[2]) && !c->name.p) {
+  // head position automata (check_prog validated them): the kHeadNfa instances of the head kernels run them
+  fei_prog_head_nfa hn{};
+  if (h.off_head_nfa) memcpy(&hn, prog + h.off_head_nfa, sizeof(hn));
+  bool head_nfa = h.off_head_nfa != 0;
+  for (uint32_t k = 0; k < h.n_slots; ++k) head_nfa = head_nfa || reinterpret_cast<const fei_prog_slot*>(prog + h.off_slots)[k].off_val_nfa != 0;
+  if ((h.off_name_dfa[0] || h.off_name_dfa[1] || h.off_name_dfa[2] || hn.off_name_nfa[0] || hn.off_name_nfa[1] || hn.off_name_nfa[2]) && !c->name.p) {
     set_error("program reads filename / id / hostname but the corpus was packed without names"); return FEI_E_STATE;
   }
   const uint32_t nq = h.n_queries;
@@ -1924,13 +2026,13 @@ int run_scan(fei_corpus* c, const uint8_t* prog, uint64_t prog_len, int compact_
       }
     }
     if (fuse) {
-      k_head_meta<true><<<meta_grid, 256, 0, s>>>(a, nullptr, nullptr);
+      (head_nfa ? k_head_meta<true, true> : k_head_meta<true, false>)<<<meta_grid, 256, 0, s>>>(a, nullptr, nullptr);
       ++launches;
     } else {
-      k_head_meta<false><<<meta_grid, 256, 0, s>>>(a, c->survivors.as<Survivor>(), d_count);
+      (head_nfa ? k_head_meta<false, true> : k_head_meta<false, false>)<<<meta_grid, 256, 0, s>>>(a, c->survivors.as<Survivor>(), d_count);
       ++launches;
       if (h.slot_mask | h.name_mask) {                         // somebody may need header text or name fields
-        k_head_parse<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(a, c->survivors.as<Survivor>(), d_count);
+        (head_nfa ? k_head_parse<true> : k_head_parse<false>)<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(a, c->survivors.as<Survivor>(), d_count);
         ++launches;
       }
     }

@@ -21,7 +21,7 @@ import numpy as np
 from .. import packer
 from ..program import (C_BODY, C_CONST, C_DATE_CMP, C_FLAGS, C_FOLDER_SET, C_NAME, C_RECBITS, C_SLOT, C_STATUS_SET, C_TS_CMP, CMP, MAX_AUX,
                        NAME_DATE_STR, NAME_FILENAME, NAME_HOST, NAME_ID, NAME_TS_STR, Cond, ProgramBuilder, const, content_automaton)
-from ..regexc import Pattern, compile_patterns
+from ..regexc import Pattern
 from . import utils as U
 
 STANDARD_FOLDERS = U.STANDARD_FOLDERS
@@ -159,7 +159,7 @@ def _eval_on_strings(values: Sequence[str], op: str, v2: Any) -> List[Any]:
         return [pat] * len(values)
     if isinstance(pat, Exception):
         return [pat] * len(values)
-    d = compile_patterns([pat])
+    d = content_automaton(pat)
     return [bool(d.run(v.encode("utf-8")) & 1) != neg for v in values]
 
 

@@ -99,8 +99,9 @@ def cached_positions(patterns: Sequence[Pattern]) -> Pna:
 
 
 def content_automaton(p: Pattern):
-    """The automaton a `content` condition runs: its DFA, or its position automaton when the DFA is refused.  Both have
-    .run(bytes) -> mask (the empty-string verdict of a content condition without with_content)."""
+    """The automaton one pattern runs on the host: its DFA, or its position automaton when the DFA is refused.  Both have
+    .run(bytes) -> mask: the empty-string verdict of a content condition without with_content, and the folder / status names
+    search judges on the host."""
     try:
         return cached_dfa([p])
     except PatternTooLarge:
@@ -235,14 +236,16 @@ def serialize_nfa(a: Pna, blob: bytearray, first_bit: int) -> int:
     return desc_off
 
 
-def _route_body(patterns: Sequence[Pattern]) -> Tuple[List[int], List[int], Optional[Pna]]:
-    """Which content patterns the body DFA takes and which go to the position automaton: (dfa indices, nfa indices, the
+def _route(patterns: Sequence[Pattern], fits, sticky: bool = False) -> Tuple[List[int], List[int], Optional[Pna]]:
+    """Which of one field's patterns its DFA takes and which go to the position automaton: (dfa indices, nfa indices, the
     automaton of the nfa ones).  The union goes to the DFA whenever it compiles and fits, exactly as without the position
-    automaton.  Otherwise every pattern whose DFA is refused on its own goes to the position automaton, and then the
-    patterns with the largest DFAs until the union of the rest fits next to the position automaton's tables."""
+    automaton.  Otherwise every pattern whose DFA is refused (or does not fit) on its own goes to the position automaton, and
+    then the patterns with the largest DFAs until the union of the rest fits.  The field's size rule is
+    fits(dfa, pna, whole): whether `dfa` fits next to position automaton `pna` (None: alone); `whole` marks the first try,
+    the union compiled with `sticky`."""
     idx = list(range(len(patterns)))
     try:
-        if _table_bytes(cached_dfa(patterns, sticky=True), SMEM_TABLE_LIMIT) <= BODY_SMEM_LIMIT:
+        if fits(cached_dfa(patterns, sticky=sticky), None, True):
             return idx, [], None
     except PatternTooLarge:
         pass
@@ -250,7 +253,7 @@ def _route_body(patterns: Sequence[Pattern]) -> Tuple[List[int], List[int], Opti
     for i in idx:
         try:
             d = cached_dfa([patterns[i]])
-            if _table_bytes(d, 0) <= BODY_SMEM_LIMIT:
+            if fits(d, None, False):
                 size[i] = d.n_states
         except PatternTooLarge:
             pass
@@ -258,16 +261,31 @@ def _route_body(patterns: Sequence[Pattern]) -> Tuple[List[int], List[int], Opti
     while True:
         nfa = [i for i in idx if i not in dfa]
         a = cached_positions([patterns[i] for i in nfa])
-        room = BODY_SMEM_LIMIT - _nfa_table_bytes(a)
         if not dfa:
             break
         try:
-            if _table_bytes(cached_dfa([patterns[i] for i in dfa]), 0) <= room:
+            if fits(cached_dfa([patterns[i] for i in dfa]), a, False):
                 break
         except PatternTooLarge:
             pass
         dfa.remove(max(dfa, key=lambda i: (size[i], i)))
     return dfa, nfa, a
+
+
+def _body_fits(d: Dfa, a: Optional[Pna], whole: bool) -> bool:
+    """Content: the DFA's tables (byte-indexed if small enough, for the union alone) and the position automaton's share the
+    body kernel's shared memory."""
+    room = BODY_SMEM_LIMIT - (_nfa_table_bytes(a) if a is not None else 0)
+    return _table_bytes(d, SMEM_TABLE_LIMIT if whole else 0) <= room
+
+
+def _head_fits(d: Dfa, a: Optional[Pna], whole: bool) -> bool:
+    """Header slots, flags and names: a DFA fits whenever it compiles."""
+    return True
+
+
+def _route_body(patterns: Sequence[Pattern]) -> Tuple[List[int], List[int], Optional[Pna]]:
+    return _route(patterns, _body_fits, sticky=True)
 
 
 def _nfa_table_bytes(a: Pna) -> int:
@@ -328,12 +346,26 @@ class ProgramBuilder:
                         ref = c.which
                 recs.append((c.kind, ref, bit, 1 if c.negate else 0, c.if_missing, c.op, c.i64, c.set64))
             qranges.append((begin, len(recs)))
-        # content patterns too large for the body DFA go to the position automaton; content bits are renumbered so that the
-        # DFA's outputs come first and the position automaton's follow
-        body_dfa, body_nfa, pna = _route_body(body.patterns) if body.patterns else ([], [], None)
-        if body_nfa:
-            new_bit = {old: new for new, old in enumerate(body_dfa + body_nfa)}
-            recs = [(kind, ref, new_bit[bit] if kind == C_BODY else bit, *rest) for kind, ref, bit, *rest in recs]
+        # patterns too large for a field's DFA go to its position automaton; each field's bits are renumbered so that the DFA's
+        # outputs come first and the position automaton's follow
+        fields = {(C_BODY, 0): body, (C_FLAGS, 0): flags, **{(C_SLOT, k): f for k, f in enumerate(slot_dfas)},
+                  **{(C_NAME, k): f for k, f in enumerate(names)}}
+        routes = {key: (_route_body(f.patterns) if key[0] == C_BODY else _route(f.patterns, _head_fits)) if f.patterns else ([], [], None)
+                  for key, f in fields.items()}
+        new_bit = {key: {old: new for new, old in enumerate(dfa + nfa)} for key, (dfa, nfa, _a) in routes.items() if nfa}
+        recs = [(kind, ref, new_bit[kind, ref][bit] if (kind, ref) in new_bit else bit, *rest) for kind, ref, bit, *rest in recs]
+        body_dfa, body_nfa, pna = routes[C_BODY, 0]
+
+        def head_field(key, direct: int) -> Tuple[int, int]:
+            """Serialise a head field: (its DFA's offset, its position automaton's), 0 for a part it does not have."""
+            f = fields[key]
+            if not f.patterns:
+                return 0, 0
+            dfa, nfa, a = routes[key]
+            if not nfa:
+                return serialize_dfa(f.compile(), blob, direct), 0
+            off_dfa = serialize_dfa(cached_dfa([f.patterns[i] for i in dfa]), blob, direct) if dfa else 0
+            return off_dfa, serialize_nfa(a, blob, len(dfa))
 
         # small head automata are stored byte-indexed (one lookup per byte in the head kernels) as long as the whole
         # program head still fits the kernels' shared-memory window; otherwise class-indexed (two lookups, smaller)
@@ -356,10 +388,15 @@ class ProgramBuilder:
                             for f, mode, _e in slots]
                 off_key = serialize_dfa(compile_patterns(key_pats), blob)          # only run over the key dictionary (k_key_lut)
                 for si, (f, mode, empty) in enumerate(slots):
-                    off_val = serialize_dfa(slot_dfas[si].compile(), blob, head_direct)
-                    struct.pack_into("<4I", blob, off_slots + 16 * si, mode, off_val, 1 if empty else 0, 0)
-            off_flags = serialize_dfa(flags.compile(), blob, head_direct) if flags.patterns else 0
-            off_names = [serialize_dfa(nf.compile(), blob, head_direct) if nf.patterns else 0 for nf in names]
+                    off_val, off_val_nfa = head_field((C_SLOT, si), head_direct)
+                    struct.pack_into("<4I", blob, off_slots + 16 * si, mode, off_val, 1 if empty else 0, off_val_nfa)
+            off_flags, off_flags_nfa = head_field((C_FLAGS, 0), head_direct)
+            off_names, off_name_nfa = zip(*[head_field((C_NAME, k), head_direct) for k in range(len(names))])
+            off_head_nfa = 0
+            if off_flags_nfa or any(off_name_nfa):         # fei_prog_head_nfa
+                _pad16(blob)
+                off_head_nfa = len(blob)
+                blob.extend(struct.pack("<8I", off_flags_nfa, *off_name_nfa, 0, 0))
             _pad16(blob)
             if len(blob) <= HEAD_SMEM_WINDOW:
                 break
@@ -377,10 +414,11 @@ class ProgramBuilder:
         if tb > BODY_SMEM_LIMIT:
             raise NotImplementedError(f"content automaton needs {tb} bytes of shared memory (limit 220 KiB)")
         _pad16(blob)
-        struct.pack_into("<22I", blob, 0, MAGIC, VERSION_NFA if off_nfa else VERSION, len(blob), len(self.queries), len(recs), off_conds,
+        version = VERSION_NFA if any(nfa for _dfa, nfa, _a in routes.values()) else VERSION
+        struct.pack_into("<22I", blob, 0, MAGIC, version, len(blob), len(self.queries), len(recs), off_conds,
                          off_queries, len(slots), off_slots, off_key, off_body, off_flags, off_names[0], off_names[1], off_names[2],
                          head_mask, body_mask, slot_mask, name_mask, head_bytes, off_names[3], off_names[4])
-        struct.pack_into("<I", blob, 88, off_nfa)
+        struct.pack_into("<2I", blob, 88, off_nfa, off_head_nfa)
         return bytes(blob)
 
 

@@ -7,7 +7,8 @@
  * of its conditions (search.py:309-331; filter.py:80-107).  Every string-valued condition is
  * one output bit of a multi-output byte DFA attached to the field it reads
  * (fei_b200/regexc): all conditions on the same field share one automaton, so a field is
- * read once no matter how many queries look at it.
+ * read once no matter how many queries look at it.  Patterns whose DFA is refused go to the field's position automaton
+ * (fei_prog_nfa) instead, which owns the field's bits above its DFA's.
  *
  * Little-endian; offsets are bytes from the start of the blob; every section is 16-byte
  * aligned so tables can be staged into shared memory with 1-D bulk copies (cp.async.bulk).
@@ -18,7 +19,9 @@
 
 #define FEI_PROG_MAGIC   0x50494546u   /* "FEIP" */
 #define FEI_PROG_VERSION 1u
-#define FEI_PROG_VERSION_NFA 2u        /* written only by programs that carry a content position automaton (fei_prog_nfa) */
+#define FEI_PROG_VERSION_NFA 2u        /* written only by programs that carry at least one position automaton (fei_prog_nfa):
+                                          content (off_body_nfa), a header slot (fei_prog_slot.off_val_nfa), flags or a name
+                                          field (off_head_nfa) */
 #define FEI_MAX_QUERIES  32
 #define FEI_MAX_SLOTS    16
 
@@ -61,18 +64,21 @@ typedef struct fei_prog_hdr {            /* 96 bytes */
                                             head kernels copy into shared memory; 0 = unknown (do not stage)              */
   uint32_t off_meta_dfa[2];              /* name fields 3 and 4: automata over the formatted timestamp / date strings        */
   uint32_t off_body_nfa;                 /* version 2 only: fei_prog_nfa of the content patterns too large for the body DFA; 0 = none */
-  uint32_t reserved;
+  uint32_t off_head_nfa;                 /* version 2 only: fei_prog_head_nfa (position automata of flags and the name fields); 0 = none */
 } fei_prog_hdr;
 
-/* Content position automaton (bit-parallel NFA, fei_b200/regexc compile_positions), for content patterns whose DFA is too
- * large.  A record is stepped per code point over a W-word bit vector D of positions (bit 0: the virtual start, set before
+/* Position automaton (bit-parallel NFA, fei_b200/regexc compile_positions), for content patterns whose DFA is too
+ * large, and for the patterns of a head field (header slot, flags, name field) whose DFA is refused.  A value is stepped per code point over a W-word bit vector D of positions (bit 0: the virtual start, set before
  * the first character only):
  *     ctx = 1 << (prev_kind * 5 + kind(c))           kinds: 0 start / end, 1 '\n', 2 word, 3 Unicode-only word, 4 other
  *     acc |= OR over accept groups a, not end-only:  (D & src_a) != 0 && (ctx_a & ctx)  ->  bit_a
  *     D    = (((D << 1) & SHIFT) | (D & SELF) | OR over follow groups g: (D & src_g) != 0 && (ctx_g & ctx) -> dst_g) & B[class(c)]
- * and at the end with next kind 0, every accept group counted.  Output bits are first_bit .. first_bit + n_patterns - 1 of the
- * content verdict; a program's body DFA (class-indexed, not sticky, when there is one) owns the bits below first_bit.
- * Every table is 16-byte aligned and the tables are contiguous from off_ascii (table_bytes): one bulk copy stages them. */
+ * and at the end with next kind 0, every accept group counted; the empty string is the reset vector finished at once.  Output
+ * bits are first_bit .. first_bit + n_patterns - 1 of the field's verdict; the field's DFA, when it has one, owns the bits below
+ * first_bit (the body DFA next to a content automaton is class-indexed and not sticky).  Every table is 16-byte aligned and the
+ * tables are contiguous from off_ascii (table_bytes): one bulk copy stages them.  The sections of head fields (slots, flags,
+ * names, fei_prog_head_nfa) lie inside [0, head_bytes), so the head kernels stage them with the rest of the head; the content
+ * one lies behind it. */
 typedef struct fei_prog_nfa {            /* 64 bytes */
   uint32_t n_words;                      /* W: 1, 2, 4 or 8 32-bit words per position vector                               */
   uint32_t n_pos;                        /* positions (bits) in use, the start bit included; <= 32 * W                      */
@@ -89,6 +95,14 @@ typedef struct fei_prog_nfa {            /* 64 bytes */
 #define FEI_NFA_MAX_CLASSES 128
 #define FEI_NFA_MAX_RANGES  4096
 #define FEI_NFA_MAX_GROUPS  64           /* follow groups, and accept groups, each */
+
+/* Position automata of flags and the name fields (fei_prog_hdr.off_head_nfa, inside [0, head_bytes)).  0 = the field has none;
+ * a field with an automaton and no DFA has off_flags_dfa / off_name_dfa / off_meta_dfa 0. */
+typedef struct fei_prog_head_nfa {       /* 32 bytes */
+  uint32_t off_flags_nfa;
+  uint32_t off_name_nfa[FEI_NAME_FIELDS];   /* indexed like FEI_C_NAME refs */
+  uint32_t reserved[2];
+} fei_prog_head_nfa;
 
 typedef struct fei_prog_dfa {            /* 64 bytes; tables follow at the given offsets            */
   uint32_t n_states, n_cols;             /* n_cols == 256: byte-indexed rows; else class-indexed     */
@@ -127,9 +141,10 @@ typedef struct fei_prog_slot {           /* 16 bytes */
                                             1: exact key, last value (search.py:117-118 "Status"; filter.py:90-91)
                                             2: every key: OR over the values of the headers dict (utils.py:333-336, the legacy
                                                substring search); the key pattern of such a slot matches every key                      */
-  uint32_t off_val_dfa;
+  uint32_t off_val_dfa;                  /* 0 = the slot has only a position automaton                                                   */
   uint32_t empty_if_missing;             /* 1: an absent header reads as "" (headers.get("Status", ""), search.py:118)                   */
-  uint32_t reserved;
+  uint32_t off_val_nfa;                  /* version 2 only: fei_prog_nfa of the slot's patterns its DFA cannot hold; 0 = none; at least
+                                            one of off_val_dfa / off_val_nfa is set                                                     */
 } fei_prog_slot;
 
 #endif /* FEISCAN_PROG_H_ */
