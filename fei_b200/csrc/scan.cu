@@ -13,8 +13,9 @@
 //          its header directory (hdir.cu: interned key + stripped value span per line; k_key_lut maps the corpus'
 //          distinct keys to the program's fields once per scan), or, for headers the directory cannot address, its
 //          text split / stripped like utils.py:113-118.  Every string condition is an output bit of a byte DFA (or of the field's
-//          position automaton, head_nfa_run, for patterns the DFA refuses; k_head_meta<kFused, true> / k_head_parse<true>); the program
-//          head (conditions + small automata) is staged into shared memory by a TMA bulk copy per CTA.
+//          position automaton, head_nfa_run, for patterns the DFA refuses; k_head_meta<kFused, true, *> / k_head_parse<true, *>); the
+//          program head (conditions + small automata + folder-set bitmaps) is staged into shared memory by a TMA bulk copy per CTA.
+//          A folder set with a folder id of 64 or above is a bitmap in the head, read by the kFolderBits instances only.
 //          Writes alive[i] = bitmask of queries whose non-content conditions all hold.
 // k_body : one warp per group of 32 records in the warp-transposed body tiles (corpus.h): each
 //          row is one contiguous coalesced request (ld.global.nc 16 B per lane); each lane walks
@@ -348,6 +349,9 @@ __device__ __forceinline__ bool cmp_i64(int64_t v, int64_t o, uint32_t op) {
     case FEI_CMP_EQ: return v == o; default: return v != o;
   }
 }
+// kFolderBits: some folder set of the program is a bitmap (folder ids of 64 and above).  Only the instances of the head kernels for
+// such programs read it; the others keep the set64 test alone, which costs the unrolled meta loop no registers.
+template <bool kFolderBits>
 __device__ __forceinline__ bool eval_meta_cond(const HeadArgs& a, uint64_t rec, const fei_prog_cond& cd, uint32_t flags_acc, int64_t wall, uint32_t fsb) {
   switch (cd.kind) {
     case FEI_C_RECBITS: {
@@ -368,7 +372,15 @@ __device__ __forceinline__ bool eval_meta_cond(const HeadArgs& a, uint64_t rec, 
         case FEI_CMP_EQ: return v == o; default: return v != o;
       }
     }
-    case FEI_C_FOLDER_SET: return (cd.set64 >> (fsb & 0xFFFFu) & 1ull) != 0;
+    case FEI_C_FOLDER_SET:
+      if constexpr (kFolderBits) {                             // set64, or the program's bitmap of the set (fei_prog_cond.off_set_words)
+        const uint32_t fid = fsb & 0xFFFFu;
+        if (!cd.off_set_words) return fid < 64u && (cd.set64 >> fid & 1ull) != 0;
+        const uint32_t* words = reinterpret_cast<const uint32_t*>(a.prog + cd.off_set_words);     // staged with the head (check_prog)
+        return fid < 32u * cd.n_set_words && (words[fid >> 5] >> (fid & 31u) & 1u) != 0;
+      } else {
+        return (cd.set64 >> (fsb & 0xFFFFu) & 1ull) != 0;
+      }
     case FEI_C_STATUS_SET: return (cd.set64 >> ((fsb >> 16) & 0xFFu) & 1ull) != 0;
     default: return true;                                      // slot / name / body: decided later
   }
@@ -446,8 +458,8 @@ __device__ __noinline__ void eval_name_fields(const NameArgs a, const fei_prog_h
 }
 
 // Phase 2 for one record: header fields (if `parse`), name fields, evaluation of the queries left in `pre`.  kHeadNfa: the
-// program has head position automata (a slot may then have no DFA).
-template <bool kHeadNfa>
+// program has head position automata (a slot may then have no DFA); kFolderBits: see eval_meta_cond.
+template <bool kHeadNfa, bool kFolderBits>
 __device__ void head_finish(const HeadArgs& a, uint64_t rec, uint32_t pre, uint32_t flags_acc, bool parse) {
   const fei_prog_hdr* ph = reinterpret_cast<const fei_prog_hdr*>(a.prog);
   const fei_prog_cond* conds = reinterpret_cast<const fei_prog_cond*>(a.prog + ph->off_conds);
@@ -530,7 +542,7 @@ __device__ void head_finish(const HeadArgs& a, uint64_t rec, uint32_t pre, uint3
         case FEI_C_NAME: r = ((name_acc[cd.ref < FEI_NAME_FIELDS ? cd.ref : 0] >> cd.bit) & 1u) != cd.negate; break;
         default:
           // meta predicates of a query in `pre` already held in k_head_meta; only a fallback field (skipped there) is still open
-          r = fallback ? eval_meta_cond(a, rec, cd, flags_acc, a.wall[rec], a.fsb[rec]) : true;
+          r = fallback ? eval_meta_cond<kFolderBits>(a, rec, cd, flags_acc, a.wall[rec], a.fsb[rec]) : true;
       }
       fallback = false;
       ok = r;
@@ -585,7 +597,7 @@ struct Survivor { uint32_t rec, pre, flags_acc; };
 
 constexpr int kMetaPer = 4;     // records per thread: the (uniform) condition fetch / decode is paid once for four records
 
-template <bool kFused, bool kHeadNfa>
+template <bool kFused, bool kHeadNfa, bool kFolderBits>
 __global__ void __launch_bounds__(256, 5) k_head_meta(HeadArgs a, Survivor* __restrict__ list, unsigned int* __restrict__ count) {
   __shared__ __align__(128) uint8_t sprog[kHeadProgSmem];
   __shared__ uint64_t bar;
@@ -624,7 +636,7 @@ __global__ void __launch_bounds__(256, 5) k_head_meta(HeadArgs a, Survivor* __re
       const fei_prog_cond cd = conds[c];
       if (cd.kind == FEI_C_SLOT && cd.if_missing == 2) { ++c; continue; }     // header-or-fallback pair: decided in phase 2
 #pragma unroll
-      for (int r = 0; r < kMetaPer; ++r) ok[r] = ok[r] && (!valid[r] || eval_meta_cond(a, base + (uint64_t)r * 256, cd, flags_acc[r], wall[r], fsb[r]));
+      for (int r = 0; r < kMetaPer; ++r) ok[r] = ok[r] && (!valid[r] || eval_meta_cond<kFolderBits>(a, base + (uint64_t)r * 256, cd, flags_acc[r], wall[r], fsb[r]));
     }
 #pragma unroll
     for (int r = 0; r < kMetaPer; ++r) if (ok[r]) pre[r] |= 1u << q;
@@ -637,7 +649,7 @@ __global__ void __launch_bounds__(256, 5) k_head_meta(HeadArgs a, Survivor* __re
       const uint64_t i = base + (uint64_t)r * 256;
       if (!valid[r]) continue;
       if ((pre[r] & later_mask) == 0) a.alive[i] = pre[r];
-      else head_finish<kHeadNfa>(a, i, pre[r], flags_acc[r], (pre[r] & ph->slot_mask) != 0);
+      else head_finish<kHeadNfa, kFolderBits>(a, i, pre[r], flags_acc[r], (pre[r] & ph->slot_mask) != 0);
     }
     return;
   }
@@ -672,7 +684,7 @@ __global__ void __launch_bounds__(256, 5) k_head_meta(HeadArgs a, Survivor* __re
   }
 }
 
-template <bool kHeadNfa>
+template <bool kHeadNfa, bool kFolderBits>
 __global__ void __launch_bounds__(256, 5) k_head_parse(HeadArgs a, const Survivor* __restrict__ list, const unsigned int* __restrict__ n_list) {
   __shared__ __align__(128) uint8_t sprog[kHeadProgSmem];
   __shared__ uint64_t bar;
@@ -684,7 +696,7 @@ __global__ void __launch_bounds__(256, 5) k_head_parse(HeadArgs a, const Survivo
   if (t >= n_surv) return;
   const fei_prog_hdr* ph = reinterpret_cast<const fei_prog_hdr*>(a.prog);
   const Survivor sv = list[t];
-  head_finish<kHeadNfa>(a, sv.rec, sv.pre, sv.flags_acc, (sv.pre & ph->slot_mask) != 0);
+  head_finish<kHeadNfa, kFolderBits>(a, sv.rec, sv.pre, sv.flags_acc, (sv.pre & ph->slot_mask) != 0);
 }
 
 // ---------------------------------------------------------------- body kernel
@@ -1933,6 +1945,14 @@ static int check_prog(const uint8_t* prog, uint64_t len) {
   }
   const fei_prog_query* qs = reinterpret_cast<const fei_prog_query*>(prog + h.off_queries);
   for (uint32_t q = 0; q < h.n_queries; ++q) if (qs[q].cond_begin > qs[q].cond_end || qs[q].cond_end > h.n_conds) { set_error("bad query range"); return FEI_E_BADARG; }
+  for (uint32_t c = 0; c < h.n_conds; ++c) {        // folder-set bitmaps: inside the blob, and inside the head the kernels stage
+    fei_prog_cond cd; memcpy(&cd, prog + h.off_conds + (uint64_t)c * sizeof(cd), sizeof(cd));
+    if (cd.kind != FEI_C_FOLDER_SET || !cd.off_set_words) continue;
+    const uint64_t end = cd.off_set_words + 4ull * cd.n_set_words;
+    if (!cd.n_set_words || cd.n_set_words > 2048 || !in(cd.off_set_words, 4ull * cd.n_set_words) || (h.head_bytes && end > h.head_bytes)) {
+      set_error("bad folder-set bitmap in program"); return FEI_E_BADARG;
+    }
+  }
   return FEI_OK;
 }
 
@@ -1966,6 +1986,13 @@ int run_scan(fei_corpus* c, const uint8_t* prog, uint64_t prog_len, int compact_
   if (h.off_head_nfa) memcpy(&hn, prog + h.off_head_nfa, sizeof(hn));
   bool head_nfa = h.off_head_nfa != 0;
   for (uint32_t k = 0; k < h.n_slots; ++k) head_nfa = head_nfa || reinterpret_cast<const fei_prog_slot*>(prog + h.off_slots)[k].off_val_nfa != 0;
+  // a folder set held as a bitmap (folder ids of 64 and above): the kFolderBits instances of the head kernels, which are
+  // instantiated only next to kHeadNfa (they run programs without head automata too)
+  bool folder_bits = false;
+  for (uint32_t k = 0; k < h.n_conds; ++k) {
+    const fei_prog_cond* cd = reinterpret_cast<const fei_prog_cond*>(prog + h.off_conds) + k;
+    folder_bits = folder_bits || (cd->kind == FEI_C_FOLDER_SET && cd->off_set_words != 0);
+  }
   if ((h.off_name_dfa[0] || h.off_name_dfa[1] || h.off_name_dfa[2] || hn.off_name_nfa[0] || hn.off_name_nfa[1] || hn.off_name_nfa[2]) && !c->name.p) {
     set_error("program reads filename / id / hostname but the corpus was packed without names"); return FEI_E_STATE;
   }
@@ -2026,13 +2053,13 @@ int run_scan(fei_corpus* c, const uint8_t* prog, uint64_t prog_len, int compact_
       }
     }
     if (fuse) {
-      (head_nfa ? k_head_meta<true, true> : k_head_meta<true, false>)<<<meta_grid, 256, 0, s>>>(a, nullptr, nullptr);
+      (folder_bits ? k_head_meta<true, true, true> : head_nfa ? k_head_meta<true, true, false> : k_head_meta<true, false, false>)<<<meta_grid, 256, 0, s>>>(a, nullptr, nullptr);
       ++launches;
     } else {
-      (head_nfa ? k_head_meta<false, true> : k_head_meta<false, false>)<<<meta_grid, 256, 0, s>>>(a, c->survivors.as<Survivor>(), d_count);
+      (folder_bits ? k_head_meta<false, true, true> : head_nfa ? k_head_meta<false, true, false> : k_head_meta<false, false, false>)<<<meta_grid, 256, 0, s>>>(a, c->survivors.as<Survivor>(), d_count);
       ++launches;
       if (h.slot_mask | h.name_mask) {                         // somebody may need header text or name fields
-        (head_nfa ? k_head_parse<true> : k_head_parse<false>)<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(a, c->survivors.as<Survivor>(), d_count);
+        (folder_bits ? k_head_parse<true, true> : head_nfa ? k_head_parse<true, false> : k_head_parse<false, false>)<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(a, c->survivors.as<Survivor>(), d_count);
         ++launches;
       }
     }

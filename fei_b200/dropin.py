@@ -8,10 +8,12 @@ replaces  memdir_tools.search.search_memories          (search.py:337)
           memdir_tools.filter.FilterManager.process_memories / run_filters   (filter.py:188, :311)
           memdir_tools.filter.MemoryFilter.matches     (filter.py:67)
           memdir_tools.memorychain.MemoryChain.validate_chain                (memorychain.py:596)
+          memdir_tools.archiver.MemoryArchiver: archive_old_memories, cleanup_memories, empty_trash,
+              apply_retention_policies, update_memory_statuses, run_maintenance   (archiver.py:205-639)
 and adds  memdir_tools.filter.apply_filters.  Names other modules already imported (`from memdir_tools.search import
 search_memories` in server.py / cli.py, the package's own re-exports) are rebound too, by identity.
-Everything else of the reference (SearchQuery objects, MemoryFilter objects, block classes, servers) is used as is:
-the GPU layer only reads their public attributes."""
+Everything else of the reference (SearchQuery objects, MemoryFilter objects, MemoryArchiver settings, block classes,
+servers) is used as is: the GPU layer only reads their public attributes."""
 from __future__ import annotations
 
 import importlib
@@ -28,6 +30,46 @@ def _rebind(orig: Any, new: Any) -> None:
         for name, val in list(d.items()):
             if val is orig:
                 d[name] = new
+
+
+_ARCHIVER_STATE = ("archive_rules", "tag_based_archiving", "retention_policies", "cleanup_rules", "archive_folder", "trash_folder",
+                   "archive_age", "trash_age")
+
+
+def _install_archiver(cls: Any, sync_base) -> None:
+    """The maintenance methods of the reference's MemoryArchiver run on the GPU against the reference object's settings.  The
+    rule lists and dicts are shared, not copied, so the default rules a stage adds land on the reference object as there."""
+    from .memdir_tools import archiver as garchiver
+
+    def gpu(ref: Any) -> "garchiver.MemoryArchiver":
+        sync_base()
+        g = garchiver.MemoryArchiver()
+        for name in _ARCHIVER_STATE:
+            setattr(g, name, getattr(ref, name))
+        return g
+
+    def archive_old_memories(self, dry_run=False):
+        return gpu(self).archive_old_memories(dry_run)
+
+    def cleanup_memories(self, dry_run=False):
+        return gpu(self).cleanup_memories(dry_run)
+
+    def empty_trash(self, age_days=None, dry_run=False):
+        return gpu(self).empty_trash(age_days, dry_run)
+
+    def apply_retention_policies(self, dry_run=False):
+        return gpu(self).apply_retention_policies(dry_run)
+
+    def update_memory_statuses(self, dry_run=False):
+        return gpu(self).update_memory_statuses(dry_run)
+
+    def run_maintenance(self, dry_run=False):
+        return {"archive": self.archive_old_memories(dry_run), "cleanup": self.cleanup_memories(dry_run),
+                "trash": self.empty_trash(dry_run=dry_run), "retention": self.apply_retention_policies(dry_run),
+                "status": self.update_memory_statuses(dry_run)}
+
+    for fn in (archive_old_memories, cleanup_memories, empty_trash, apply_retention_policies, update_memory_statuses, run_maintenance):
+        setattr(cls, fn.__name__, fn)
 
 
 def install(package: str = "memdir_tools") -> None:
@@ -83,6 +125,12 @@ def install(package: str = "memdir_tools") -> None:
     _rebind(ref_filter.run_filters, run_filters)
     ref_filter.run_filters = run_filters
     ref_filter.apply_filters = apply_filters
+    try:
+        ref_arch = importlib.import_module(f"{package}.archiver")
+    except ImportError:
+        ref_arch = None
+    if ref_arch is not None:
+        _install_archiver(ref_arch.MemoryArchiver, _sync_base)
     try:
         ref_chain = importlib.import_module(f"{package}.memorychain")
     except Exception:                                        # the reference module needs `requests`

@@ -52,10 +52,9 @@ class MemdirFolderManager:
                     stats["subfolders"].append(sub)
             if not segs:
                 return stats
-            # which packed folder ids are in play (one bit per folder id, as search does for folder restrictions)
+            # which packed folder ids are in play (one bit per folder id, as search does for folder restrictions; ids of 64 and
+            # above go into the program as a bitmap)
             folder_ids = sorted({int(pm.arrays["fsb"][lo]) & 0xFFFF for _f, _s, lo, _hi in segs})
-            if max(folder_ids) >= 64:
-                raise NotImplementedError("more than 64 folders in one Memdir are not supported by the packed folder set")
             fset = 0
             for fid in folder_ids:
                 fset |= 1 << fid

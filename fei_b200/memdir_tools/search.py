@@ -219,8 +219,6 @@ def _compile_one(field: Any, op: str, v2: Any, include_content: bool, pm) -> Lis
     if low in ("folder", "status", "maildir_status"):
         names = pm.folders if low == "folder" else U.STANDARD_FOLDERS
         ids = [pm.folder_ids[f] for f in names] if low == "folder" else list(range(len(names)))      # packed folder ids are stable, not positions
-        if ids and max(ids) >= 64:
-            raise NotImplementedError("folder predicates on more than 64 folders")
         verdicts = _eval_on_strings(names, op, v2)
         if any(isinstance(v, Exception) for v in verdicts):
             return [_Raises(next(v for v in verdicts if isinstance(v, Exception)), None)]

@@ -41,7 +41,7 @@ class Cond:
     which: int = 0               # name field
     op: int = 0                  # date_cmp
     i64: int = 0
-    set64: int = 0
+    set64: int = 0               # folder / status set: bit k = id k (a folder set may hold ids of 64 and above)
     value: bool = False          # const
 
 
@@ -380,6 +380,12 @@ class ProgramBuilder:
             for a, b in qranges:
                 blob.extend(struct.pack("<4I", a, b, 0, 0))
             _pad16(blob)
+            for ci, (kind, *_rest, set64) in enumerate(recs):
+                if kind == C_FOLDER_SET and set64 >> 64:      # a folder id of 64 or above: the set as a bitmap (fei_prog_cond.off_set_words)
+                    n_words = (set64.bit_length() + 31) // 32
+                    struct.pack_into("<2I", blob, off_conds + 32 * ci + 24, len(blob), n_words)
+                    blob.extend(set64.to_bytes(4 * n_words, "little"))
+                    _pad16(blob)
             off_slots = len(blob)
             blob.extend(b"\0" * (16 * len(slots)))
             off_key = 0

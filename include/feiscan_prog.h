@@ -33,7 +33,8 @@ enum {
   FEI_C_FLAGS      = 3,  /* output `bit` of the flags DFA          (search.py:105-106, filter.py:92-93)    */
   FEI_C_NAME       = 4,  /* output `bit` of name-field `ref` DFA: 0 filename, 1 unique_id, 2 hostname      */
   FEI_C_DATE_CMP   = 5,  /* wall-clock microseconds `cmp_op` i64   (search.py:107-108, :166-234)           */
-  FEI_C_FOLDER_SET = 6,  /* (set64 >> folder_id) & 1               (host-evaluated per distinct folder)    */
+  FEI_C_FOLDER_SET = 6,  /* (set64 >> folder_id) & 1               (host-evaluated per distinct folder); with
+                            off_set_words != 0 the set is that bitmap instead (folder ids of 64 and above)       */
   FEI_C_STATUS_SET = 7,  /* (set64 >> status_id) & 1                                                        */
   FEI_C_RECBITS    = 8,  /* aux column `ref` of the corpus (fei_corpus_set_aux): one host-computed verdict byte per
                             record, for values only Python can judge (per-record dateutil parses of Due / Created /
@@ -131,7 +132,12 @@ typedef struct fei_prog_cond {           /* 32 bytes */
   uint8_t pad[2];
   int64_t i64;
   uint64_t set64;
-  uint64_t pad2;
+  uint32_t off_set_words;                /* FEI_C_FOLDER_SET only: 0 = the set is set64 (folder ids 0..63).  Else the byte offset of
+                                            the set as a bitmap, uint32_t[n_set_words], folder id k = bit k % 32 of word k / 32; ids
+                                            at or above 32 * n_set_words are outside the set.  16-byte aligned and inside
+                                            [0, head_bytes), so the head kernels stage it with the conditions.  program.py writes it
+                                            only when the set holds a folder id of 64 or above; set64 then carries ids 0..63 too. */
+  uint32_t n_set_words;                  /* ceil((largest folder id in the set + 1) / 32) */
 } fei_prog_cond;
 
 typedef struct fei_prog_query { uint32_t cond_begin, cond_end, reserved0, reserved1; } fei_prog_query;
