@@ -1,12 +1,10 @@
-// Canonical JSON of a Memorychain block's hashed fields, as produced by
-//   json.dumps({...ten fields...}, sort_keys=True)          (memdir_tools/memorychain.py:117-128)
-// i.e. keys in sorted order, separators ", " and ": ", ensure_ascii=True, Python float repr.
-// Host C++ (multi-threaded); the GPU then hashes the texts (chain.cu).
+// Canonical JSON of Memorychain blocks on the host, multi-threaded; the GPU then hashes the texts (chain.cu).  Every block
+// goes through the writer in jsonfmt.cuh, the source chain.cu's k_json_* kernels format the resident image with, so
+// one-shot and resident validation hash the same bytes.
 #include "common.h"
 #include "chain_json.h"
+#include "jsonfmt.cuh"
 
-#include <charconv>
-#include <cmath>
 #include <cstring>
 #include <cstdlib>
 #include <thread>
@@ -14,149 +12,6 @@
 #include <algorithm>
 
 namespace fei {
-
-static const char* const kKeys[FEI_CHAIN_NCOLS] = {
-    "difficulty", "index", "memory_id", "nonce", "previous_hash",
-    "proposer_node", "responsible_node", "solver_node", "task_state", "timestamp"};
-
-namespace {
-
-// Raw writer: the caller guarantees room (block_bound) before every block, so a byte costs a store, not a capacity check.
-struct Out {
-  uint8_t* p;
-  void put(char c) { *p++ = (uint8_t)c; }
-  void put(const char* s, size_t n) { memcpy(p, s, n); p += n; }
-  void lit(const char* s) { put(s, strlen(s)); }
-};
-
-inline void put_u4(Out& o, unsigned cp) {  // \uXXXX, lowercase hex like json.encoder
-  static const char hx[] = "0123456789abcdef";
-  char b[6] = {'\\', 'u', hx[(cp >> 12) & 15], hx[(cp >> 8) & 15], hx[(cp >> 4) & 15], hx[cp & 15]};
-  o.put(b, 6);
-}
-
-// py_encode_basestring_ascii: everything outside ' '..'~' plus '"' and '\\' is escaped.
-// Input is UTF-8 (lone surrogates arrive as 3-byte "surrogatepass" sequences).
-void put_json_string(Out& o, const uint8_t* s, size_t n) {
-  o.put('"');
-  size_t i = 0;
-  while (i < n) {
-    unsigned c = s[i];
-    if (c < 0x80) {
-      ++i;
-      switch (c) {
-        case '"': o.lit("\\\""); break;
-        case '\\': o.lit("\\\\"); break;
-        case '\n': o.lit("\\n"); break;
-        case '\r': o.lit("\\r"); break;
-        case '\t': o.lit("\\t"); break;
-        case '\b': o.lit("\\b"); break;
-        case '\f': o.lit("\\f"); break;
-        default:
-          if (c >= 0x20 && c <= 0x7E) o.put((char)c); else put_u4(o, c);
-      }
-      continue;
-    }
-    unsigned cp; int len;
-    if ((c & 0xE0) == 0xC0) { cp = c & 0x1F; len = 2; }
-    else if ((c & 0xF0) == 0xE0) { cp = c & 0x0F; len = 3; }
-    else { cp = c & 0x07; len = 4; }
-    for (int k = 1; k < len && i + k < n; ++k) cp = (cp << 6) | (s[i + k] & 0x3F);
-    i += len;
-    if (cp >= 0x10000) {
-      unsigned v = cp - 0x10000;
-      put_u4(o, 0xD800 | (v >> 10));
-      put_u4(o, 0xDC00 | (v & 0x3FF));
-    } else {
-      put_u4(o, cp);
-    }
-  }
-  o.put('"');
-}
-
-void put_int(Out& o, int64_t v) {
-  char b[24];
-  auto r = std::to_chars(b, b + sizeof(b), v);
-  o.put(b, r.ptr - b);
-}
-
-// float.__repr__ (Python/pystrtod.c format_float_short, mode 'r'): shortest digits that
-// round-trip; exponent form iff decpt <= -4 or decpt > 16; ".0" appended to integers;
-// exponent has at least two digits.  json.dumps spells the non-finite values
-// NaN / Infinity / -Infinity (allow_nan=True).
-void put_float(Out& o, double x) {
-  if (std::isnan(x)) { o.lit("NaN"); return; }
-  if (std::isinf(x)) { o.lit(x > 0 ? "Infinity" : "-Infinity"); return; }
-  if (x == 0.0) { o.lit(std::signbit(x) ? "-0.0" : "0.0"); return; }
-  char b[48];
-  auto r = std::to_chars(b, b + sizeof(b), x, std::chars_format::scientific);  // d[.ddd]e[+-]XX shortest
-  char* p = b;
-  bool neg = false;
-  if (*p == '-') { neg = true; ++p; }
-  char digits[24]; int nd = 0;
-  while (p < r.ptr && *p != 'e') { if (*p != '.') digits[nd++] = *p; ++p; }
-  int exp10 = 0;
-  if (p < r.ptr && *p == 'e') {
-    ++p; bool eneg = false;
-    if (*p == '+') ++p; else if (*p == '-') { eneg = true; ++p; }
-    while (p < r.ptr) { exp10 = exp10 * 10 + (*p - '0'); ++p; }
-    if (eneg) exp10 = -exp10;
-  }
-  while (nd > 1 && digits[nd - 1] == '0') --nd;   // to_chars never pads, but be safe
-  int decpt = exp10 + 1;
-  if (neg) o.put('-');
-  if (decpt <= -4 || decpt > 16) {
-    o.put(digits[0]);
-    if (nd > 1) { o.put('.'); o.put(digits + 1, nd - 1); }
-    o.put('e');
-    int e = decpt - 1;
-    o.put(e < 0 ? '-' : '+');
-    if (e < 0) e = -e;
-    char eb[8]; int ne = 0;
-    do { eb[ne++] = (char)('0' + e % 10); e /= 10; } while (e);
-    if (ne < 2) eb[ne++] = '0';
-    while (ne) o.put(eb[--ne]);
-  } else if (decpt <= 0) {
-    o.lit("0.");
-    for (int k = 0; k < -decpt; ++k) o.put('0');
-    o.put(digits, nd);
-  } else if (decpt >= nd) {
-    o.put(digits, nd);
-    for (int k = nd; k < decpt; ++k) o.put('0');
-    o.lit(".0");
-  } else {
-    o.put(digits, decpt);
-    o.put('.');
-    o.put(digits + decpt, nd - decpt);
-  }
-}
-
-int put_value(Out& o, const fei_json_col& c, uint64_t i) {
-  int tag = c.tag ? c.tag[i] : c.uniform_tag;
-  switch (tag) {
-    case FEI_J_NULL: o.lit("null"); return 0;
-    case FEI_J_TRUE: o.lit("true"); return 0;
-    case FEI_J_FALSE: o.lit("false"); return 0;
-    case FEI_J_INT: put_int(o, (int64_t)c.num[i]); return 0;
-    case FEI_J_FLOAT: { double d; memcpy(&d, &c.num[i], 8); put_float(o, d); return 0; }
-    case FEI_J_STR: put_json_string(o, c.str + c.str_off[i], c.str_off[i + 1] - c.str_off[i]); return 0;
-    case FEI_J_BIGINT: o.put((const char*)c.str + c.str_off[i], c.str_off[i + 1] - c.str_off[i]); return 0;
-    default: return -1;
-  }
-}
-
-int put_block(Out& o, const fei_json_col* cols, uint64_t i) {
-  o.put('{');
-  for (int k = 0; k < FEI_CHAIN_NCOLS; ++k) {
-    if (k) o.lit(", ");
-    o.put('"'); o.lit(kKeys[k]); o.lit("\": ");
-    if (put_value(o, cols[k], i) != 0) return -1;
-  }
-  o.put('}');
-  return 0;
-}
-
-}  // namespace
 
 // upper bound of one block's text: every string byte can become a 6-byte \\uXXXX escape (a 4-byte character two of them)
 static size_t block_bound(const fei_json_col* cols, uint64_t i) {
@@ -169,10 +24,17 @@ static size_t block_bound(const fei_json_col* cols, uint64_t i) {
   return b;
 }
 
+// One block's text at dst; returns its end, or nullptr on an unsupported tag.  flatten inlines the whole writer so the sink's
+// pointer can live in a register; otherwise every byte store, which may alias the pointer, forces a store and reload of it.
+__attribute__((flatten)) static uint8_t* write_block(uint8_t* dst, const fei_json_col* cols, uint64_t i) {
+  feijson::WriteSink o{dst};
+  return feijson::put_block(o, cols, i) == 0 ? o.p : nullptr;
+}
+
 int serialize_chain_cols(const fei_json_col* cols, uint64_t n, ByteVec& msgs, std::vector<uint64_t>& off) {
   for (int k = 0; k < FEI_CHAIN_NCOLS; ++k) {
     const fei_json_col& c = cols[k];
-    if (!c.tag && (c.uniform_tag < FEI_J_NULL || c.uniform_tag > FEI_J_BIGINT)) { set_error("column %d (%s): bad uniform tag %d", k, kKeys[k], c.uniform_tag); return FEI_E_BADARG; }
+    if (!c.tag && (c.uniform_tag < FEI_J_NULL || c.uniform_tag > FEI_J_BIGINT)) { set_error("column %d (%s): bad uniform tag %d", k, feijson::key_name(k), c.uniform_tag); return FEI_E_BADARG; }
   }
   unsigned hw = std::thread::hardware_concurrency();
   unsigned nt = (unsigned)std::min<uint64_t>(std::min(std::max(1u, hw), 32u), std::max<uint64_t>(1, n / 4096));
@@ -195,9 +57,9 @@ int serialize_chain_cols(const fei_json_col* cols, uint64_t n, ByteVec& msgs, st
         if (!nb) { rc[t] = -2; return; }
         pt.buf = nb; pt.cap = ncap;
       }
-      Out o{pt.buf + pt.len};
-      if (put_block(o, cols, i) != 0) { rc[t] = -1; return; }
-      const size_t wrote = (size_t)(o.p - (pt.buf + pt.len));
+      const uint8_t* end = write_block(pt.buf + pt.len, cols, i);
+      if (!end) { rc[t] = -1; return; }
+      const size_t wrote = (size_t)(end - (pt.buf + pt.len));
       off[i + 1] = wrote;                                       // length for now; prefix-summed below
       pt.len += wrote;
     }

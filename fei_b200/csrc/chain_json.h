@@ -1,4 +1,4 @@
-// Host canonical-JSON serialiser for Memorychain blocks (chain_json.cpp).
+// Threaded host driver for the canonical-JSON writer of Memorychain blocks (jsonfmt.cuh), in chain_json.cpp.
 #pragma once
 #include <stdint.h>
 #include <vector>

@@ -2,7 +2,7 @@
 //   json.dumps({...ten fields...}, sort_keys=True)          (memdir_tools/memorychain.py:117-128)
 // keys in sorted order, separators ", " and ": ", ensure_ascii=True, Python float repr (shortest digits that round-trip:
 // Ryu, U. Adams, PLDI 2018; then float.__repr__'s layout rules, Python/pystrtod.c format_float_short mode 'r').
-// The same source formats the column form on the GPU (chain.cu k_json_*) and on the host (chain_json.cpp, tests).
+// The same source formats the column form on the GPU (chain.cu k_json_*) and on the host (chain_json.cpp).
 #pragma once
 #include <stdint.h>
 #include <string.h>

@@ -145,10 +145,9 @@ _OPTIONAL = ("task_state", "difficulty", "solver_node")
 _get_dict = attrgetter("__dict__")
 
 
-def _extract(blocks: Sequence[Any]) -> Optional[List[tuple]]:
-    """Fast attribute extraction: when every block is a plain instance of one class whose hashed fields are ordinary
-    instance attributes, read them straight out of the instance dicts (C speed, no descriptor protocol).
-    Returns 11 tuples (7 direct, hash, 3 optional) or None when the generic getattr path must be used."""
+def _plain_hash_key(blocks: Sequence[Any]) -> Optional[str]:
+    """The instance-dict key of the stored hash when every block is a plain instance of one class whose hashed fields are
+    ordinary instance attributes, else None: the one test both fast column paths (_extract, chain_columns_native) share."""
     kinds = set(map(type, blocks))
     if len(kinds) != 1:
         return None
@@ -162,6 +161,16 @@ def _extract(blocks: Sequence[Any]) -> Optional[List[tuple]]:
         return None
     if any(hasattr(cls, k) for k in _DIRECT + _OPTIONAL) or hasattr(cls, "__getattr__"):
         return None                              # class-level attributes / descriptors / dynamic lookup: use getattr
+    return hash_key
+
+
+def _extract(blocks: Sequence[Any]) -> Optional[List[tuple]]:
+    """Fast attribute extraction: when the blocks are plain (_plain_hash_key), read the hashed fields straight out of the
+    instance dicts (C speed, no descriptor protocol).
+    Returns 11 tuples (7 direct, hash, 3 optional) or None when the generic getattr path must be used."""
+    hash_key = _plain_hash_key(blocks)
+    if hash_key is None:
+        return None
     try:
         rows = list(map(itemgetter(*_DIRECT, hash_key, *_OPTIONAL), map(_get_dict, blocks)))
     except (AttributeError, KeyError):           # __slots__ classes, blocks without task fields (getattr(..., None))
@@ -193,21 +202,11 @@ _NATIVE_NAMES = {"memory_id": "memory_data"}          # hashed field -> instance
 
 def chain_columns_native(blocks: Sequence[Any]) -> Optional[Tuple[List[_Col], np.ndarray, np.ndarray]]:
     """The ten hashed columns + the stored-hash blob through the C helper, or None when the blocks are not plain enough
-    for it (then chain_columns decides).  Same class test as _extract: one class, ordinary instance attributes."""
+    for it (then chain_columns decides)."""
     if _fastcols is None or not blocks:
         return None
-    kinds = set(map(type, blocks))
-    if len(kinds) != 1:
-        return None
-    cls = kinds.pop()
-    hash_key = "hash"
-    if isinstance(getattr(cls, "hash", None), property):
-        if cls is not MemoryBlock and cls is not _TrackedBlock:
-            return None
-        hash_key = "_hash"
-    elif hasattr(cls, "hash"):
-        return None
-    if any(hasattr(cls, k) for k in _DIRECT + _OPTIONAL) or hasattr(cls, "__getattr__"):
+    hash_key = _plain_hash_key(blocks)
+    if hash_key is None:
         return None
     names = tuple(_NATIVE_NAMES.get(k, k) for k in HASHED_FIELDS) + (hash_key,)
     out = _fastcols.columns(blocks if isinstance(blocks, list) else list(blocks), names, HASHED_FIELDS.index("memory_id"))

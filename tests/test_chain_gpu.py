@@ -251,7 +251,7 @@ def test_resident_chain_tracks_mutations(gpu, caplog):
 
 def test_gpu_canonical_json_matches_reference_kats(gpu, chain_golden):
     """fei_chain_load_cols: the column form serialised on the GPU (incl. Python's shortest round-trip float repr, ensure_ascii
-    escapes, big ints) gives the reference's digests for every golden single-block vector."""
+    escapes, big ints) gives the oracle's json.dumps text and the reference's digest for every golden single-block vector."""
     import ctypes as C
     from fei_b200 import _abi
     from fei_b200.memdir_tools import memorychain as mc
@@ -270,7 +270,7 @@ def test_gpu_canonical_json_matches_reference_kats(gpu, chain_golden):
     _abi.check(_abi.lib().fei_chain_fetch(h, 0, n, _abi.ptr(buf), buf.size, _abi.ptr(off), None, None))
     _abi.lib().fei_chain_destroy(h)
     for i, b in enumerate(blocks):
-        assert bytes(buf[int(off[i]):int(off[i + 1])]) == mc.canonical_texts([b])[0], chain_golden["single"][i]["name"]
+        assert bytes(buf[int(off[i]):int(off[i + 1])]) == co.block_text(b).encode(), chain_golden["single"][i]["name"]
         assert bytes(dig[i]).hex() == co.block_hash(b), chain_golden["single"][i]["name"]
 
 
