@@ -112,6 +112,7 @@ _SIGS = {
     "fei_corpus_token_histogram": (C.c_int, [_P, _P, _U64, C.c_uint8, _P, _U64, _P, _P, _P, _U64, _P]),
     "fei_corpus_slot_values": (C.c_int, [_P, _P, _U64, _P, _P, _P, _U64]),
     "fei_corpus_set_aux": (C.c_int, [_P, C.c_uint32, _P, _U64]),
+    "fei_corpus_tag_edit": (C.c_int, [_P, _P, _U64, C.c_uint32, _P, _P, C.c_uint32, _P, _U64, _P, _P, _U64, _P, _P]),
     "fei_chain_validate_msgs": (C.c_int, [_P, _P, _P, _P, _P, _P, _U64, _U64, _P, _P, _P]),
     "fei_chain_validate_cols": (C.c_int, [_P, _P, _P, _U64, _U64, _P, _P, _P, _P, _U64, _P]),
     "fei_chain_create": (C.c_int, [_P]),

@@ -183,6 +183,34 @@ class Corpus:
         _abi.check(rc)
         return present[:n].astype(bool), off, blob[:int(off[n])]
 
+    TAG_OPS = {"add": 0, "remove": 1, "replace": 2}
+
+    def tag_edit(self, prog: bytes, operation: str, tags: Sequence[bytes]):
+        """The records of `prog`'s query whose `Tags` multiset `operation` changes (fei_corpus_tag_edit: the tag edit of
+        folders.py:483-587; header field 0 of `prog` is the exact key Tags, field 1 the exact key Subject).  Returns
+        (global indices, [(Subject bytes or None, old tags bytes, new tags bytes)]) in corpus order."""
+        blob = b"".join(tags)
+        toff = np.zeros(len(tags) + 1, dtype=np.uint64)
+        toff[1:] = np.cumsum([len(t) for t in tags], dtype=np.uint64)
+        src = np.frombuffer(blob, dtype=np.uint8) if blob else np.zeros(1, dtype=np.uint8)
+        l = _abi.lib()
+        cap, text_cap = max(1, self.n), 64 * max(1, self.n)       # an exact retry below when the text does not fit
+        while True:
+            rec = np.empty(cap, dtype=np.uint64); text = np.empty(text_cap, dtype=np.uint8)
+            off = np.empty(3 * cap + 1, dtype=np.uint64); has = np.empty(cap, dtype=np.uint8)
+            m = C.c_uint64()
+            rc = l.fei_corpus_tag_edit(self._h, prog, len(prog), self.TAG_OPS[operation], _abi.ptr(src), _abi.ptr(toff), len(tags),
+                                       _abi.ptr(rec), cap, C.byref(m), _abi.ptr(text), text_cap, _abi.ptr(off), _abi.ptr(has))
+            if rc != _abi.FEI_E_CAPACITY:
+                break
+            cap, text_cap = max(1, m.value), max(1, int(off[0]))
+        _abi.check(rc)
+        k = m.value
+        raw = text[:int(off[3 * k])].tobytes()
+        o = off[:3 * k + 1].tolist()
+        out = [(raw[o[3 * j]:o[3 * j + 1]] if has[j] else None, raw[o[3 * j + 1]:o[3 * j + 2]], raw[o[3 * j + 2]:o[3 * j + 3]]) for j in range(k)]
+        return rec[:k].copy(), out
+
     def set_aux(self, k: int, verdicts: Optional[np.ndarray]) -> None:
         """Aux column k: one host-computed verdict byte per record, read by C_RECBITS conditions (fei_corpus_set_aux)."""
         if verdicts is None:

@@ -2568,3 +2568,239 @@ extern "C" int fei_corpus_set_aux(fei_corpus* c, uint32_t k, const uint8_t* byte
   c->aux_n[k] = n;
   return FEI_OK;
 }
+
+// ---------------------------------------------------------------- bulk tag edit (MemdirFolderManager.bulk_tag_folder)
+// folders.py:483-587, per record of the selected directories:
+//     existing = [t.strip() for t in headers["Tags"].split(",")] if "Tags" in headers else []
+//     updated  = existing + [t for t in tags if t not in existing]    (add)
+//              | [t for t in existing if t not in tags]              (remove)
+//              | tags                                                (replace)
+//     affected iff sorted(existing) != sorted(updated); it reports Subject, ", ".join(existing) and ", ".join(updated)
+// k_tag_edit_measure decides every selected record (one thread each; Tags = slot 0 and Subject = slot 1 of the program, exact
+// keys) and sizes its three strings; two exclusive scans place the affected records and their bytes; k_tag_edit_write writes
+// them.  Nothing else of a record leaves the device: the file rewrite is the host's, for the affected records only.
+namespace fei {
+constexpr uint32_t kTagOpsMax = 64, kTagBytesMax = 4096;
+struct TagOps {                                   // the operands, staged in shared memory by every CTA
+  uint32_t op, n_tags, n_dist, pad;
+  uint32_t off[kTagOpsMax + 1];                   // operand k = bytes[off[k] .. off[k+1])
+  uint16_t dist[kTagOpsMax], mult[kTagOpsMax];    // replace: each distinct operand (its first index) and how often it occurs
+  uint8_t bytes[kTagBytesMax];
+};
+static_assert(sizeof(TagOps) % 4 == 0, "TagOps is staged word by word");
+
+struct TagEditArgs {
+  const uint8_t* prog; const uint8_t* hdr; const uint64_t* hdr_off; const uint2* hdir; const uint64_t* hdir_off;
+  const uint32_t* key_lut; const uint32_t* alive; uint64_t n; const TagOps* ops;
+};
+struct TagRecord { const uint8_t* tags; const uint8_t* subj; uint32_t tags_len, subj_len; bool has_tags, has_subj; };
+// A record's header lines with the key masks shifted by `slot`: header_lookup<1> then reads program slot `slot` (one lookup per
+// field keeps the value arrays of header_lookup in registers).
+template <class Lines>
+struct SlotLines : Lines {
+  uint32_t slot;
+  __device__ __forceinline__ uint32_t key_mask() const { return Lines::key_mask() >> slot; }
+};
+
+__device__ __forceinline__ TagRecord tag_record(const TagEditArgs& a, uint64_t rec) {
+  const fei_prog_hdr* ph = reinterpret_cast<const fei_prog_hdr*>(a.prog);
+  const uint8_t* h = a.hdr + a.hdr_off[rec];
+  const uint2* ent = a.hdir + a.hdir_off[rec];
+  const uint32_t n_ent = (uint32_t)(a.hdir_off[rec + 1] - a.hdir_off[rec]);
+  const bool text = text_record(ent, n_ent);
+  auto mode = [](int) { return 1u; };                           // exact keys, the last line wins
+  auto lookup = [&](uint32_t slot, uint32_t* voff, uint32_t* vlen) {
+    return text ? header_lookup<1>(SlotLines<TextLines>{{h, h, a.hdr + a.hdr_off[rec + 1], a.prog, ph->off_key_dfa, false}, slot}, mode, voff, vlen, no_values)
+                : header_lookup<1>(SlotLines<DirLines>{{ent, n_ent, a.key_lut}, slot}, mode, voff, vlen, no_values);
+  };
+  uint32_t toff = 0, tlen = 0, soff = 0, slen = 0;
+  const bool has_tags = lookup(0, &toff, &tlen) != 0, has_subj = lookup(1, &soff, &slen) != 0;
+  return TagRecord{h + toff, h + soff, tlen, slen, has_tags, has_subj};
+}
+
+// str.split(",") of a value, every piece strip()ped: f(piece, length) for each until it returns true (then true)
+template <class F>
+__device__ __forceinline__ bool any_piece(const uint8_t* v, uint32_t len, F f) {
+  for (uint32_t pos = 0;;) {
+    uint32_t end = pos;
+    while (end < len && v[end] != ',') ++end;
+    const uint8_t* p = v + pos; const uint8_t* e = v + end;
+    strip_span(p, e);
+    if (f(p, (uint32_t)(e - p))) return true;
+    if (end >= len) return false;
+    pos = end + 1;
+  }
+}
+__device__ __forceinline__ bool same_bytes(const uint8_t* p, uint32_t lp, const uint8_t* q, uint32_t lq) {
+  if (lp != lq) return false;
+  for (uint32_t k = 0; k < lp; ++k) if (p[k] != q[k]) return false;
+  return true;
+}
+__device__ __forceinline__ bool in_existing(const TagRecord& r, const uint8_t* p, uint32_t l) {
+  return r.has_tags && any_piece(r.tags, r.tags_len, [&](const uint8_t* q, uint32_t lq) { return same_bytes(p, l, q, lq); });
+}
+__device__ __forceinline__ bool in_operands(const TagOps& o, const uint8_t* p, uint32_t l) {
+  for (uint32_t k = 0; k < o.n_tags; ++k) if (same_bytes(p, l, o.bytes + o.off[k], o.off[k + 1] - o.off[k])) return true;
+  return false;
+}
+
+// sorted(existing) != sorted(updated)
+__device__ __forceinline__ bool tag_edit_changes(const TagOps& o, const TagRecord& r) {
+  if (o.op == 0) {                                               // add: some operand is not among the pieces
+    for (uint32_t k = 0; k < o.n_tags; ++k) if (!in_existing(r, o.bytes + o.off[k], o.off[k + 1] - o.off[k])) return true;
+    return false;
+  }
+  if (o.op == 1)                                                 // remove: some piece is an operand
+    return r.has_tags && any_piece(r.tags, r.tags_len, [&](const uint8_t* p, uint32_t l) { return in_operands(o, p, l); });
+  uint32_t pieces = 0;                                           // replace: the multisets differ
+  if (r.has_tags) any_piece(r.tags, r.tags_len, [&](const uint8_t*, uint32_t) { ++pieces; return false; });
+  if (pieces != o.n_tags) return true;
+  for (uint32_t d = 0; d < o.n_dist; ++d) {                      // equal sizes: equal iff every distinct operand occurs as often
+    const uint8_t* t = o.bytes + o.off[o.dist[d]];
+    const uint32_t lt = o.off[o.dist[d] + 1] - o.off[o.dist[d]];
+    uint32_t cnt = 0;
+    any_piece(r.tags, r.tags_len, [&](const uint8_t* p, uint32_t l) { cnt += same_bytes(p, l, t, lt) ? 1u : 0u; return false; });
+    if (cnt != o.mult[d]) return true;
+  }
+  return false;
+}
+
+struct CountSink { uint32_t n = 0; __device__ void put(const uint8_t*, uint32_t l) { n += l; } };
+struct CopySink { uint8_t* d; __device__ void put(const uint8_t* p, uint32_t l) { for (uint32_t k = 0; k < l; ++k) *d++ = p[k]; } };
+template <class Sink>
+struct Joiner {                                                  // ", ".join
+  Sink& s; bool first = true;
+  __device__ void put(const uint8_t* p, uint32_t l) {
+    if (!first) { const uint8_t sep[2] = {',', ' '}; s.put(sep, 2); }
+    first = false; s.put(p, l);
+  }
+};
+template <class Sink>
+__device__ __forceinline__ void emit_old_tags(Sink& s, const TagRecord& r) {
+  Joiner<Sink> j{s};
+  if (r.has_tags) any_piece(r.tags, r.tags_len, [&](const uint8_t* p, uint32_t l) { j.put(p, l); return false; });
+}
+template <class Sink>
+__device__ __forceinline__ void emit_new_tags(Sink& s, const TagOps& o, const TagRecord& r) {
+  Joiner<Sink> j{s};
+  if (o.op != 2 && r.has_tags)                                   // add keeps every piece, remove those that are not operands
+    any_piece(r.tags, r.tags_len, [&](const uint8_t* p, uint32_t l) { if (o.op == 0 || !in_operands(o, p, l)) j.put(p, l); return false; });
+  if (o.op == 1) return;
+  for (uint32_t k = 0; k < o.n_tags; ++k) {                      // add: the operands not among the pieces; replace: all of them
+    const uint8_t* t = o.bytes + o.off[k];
+    const uint32_t lt = o.off[k + 1] - o.off[k];
+    if (o.op == 2 || !in_existing(r, t, lt)) j.put(t, lt);
+  }
+}
+
+__device__ __forceinline__ void stage_tag_ops(const TagOps* g, TagOps& s) {
+  const uint32_t* src = reinterpret_cast<const uint32_t*>(g);
+  uint32_t* dst = reinterpret_cast<uint32_t*>(&s);
+  for (uint32_t k = threadIdx.x; k < sizeof(TagOps) / 4; k += blockDim.x) dst[k] = src[k];
+  __syncthreads();
+}
+
+__global__ void __launch_bounds__(256) k_tag_edit_measure(TagEditArgs a, uint32_t* __restrict__ changed, uint32_t* __restrict__ bytes) {
+  __shared__ TagOps ops;
+  stage_tag_ops(a.ops, ops);
+  const uint64_t rec = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
+  if (rec >= a.n) return;
+  uint32_t hit = 0, len = 0;
+  if (a.alive[rec] & 1u) {
+    const TagRecord r = tag_record(a, rec);
+    if (tag_edit_changes(ops, r)) {
+      CountSink cs;
+      emit_old_tags(cs, r);
+      emit_new_tags(cs, ops, r);
+      hit = 1; len = cs.n + (r.has_subj ? r.subj_len : 0u);
+    }
+  }
+  changed[rec] = hit; bytes[rec] = len;
+}
+
+__global__ void __launch_bounds__(256) k_tag_edit_write(TagEditArgs a, const uint32_t* __restrict__ changed, const uint64_t* __restrict__ pos,
+                                                        const uint64_t* __restrict__ off, uint64_t global_base, uint64_t* __restrict__ rec_out,
+                                                        uint64_t* __restrict__ text_off, uint8_t* __restrict__ has_subject, uint8_t* __restrict__ text) {
+  __shared__ TagOps ops;
+  stage_tag_ops(a.ops, ops);
+  const uint64_t rec = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
+  if (rec >= a.n || !changed[rec]) return;
+  const TagRecord r = tag_record(a, rec);
+  const uint64_t j = pos[rec], o = off[rec];
+  CopySink s{text + o};
+  if (r.has_subj) s.put(r.subj, r.subj_len);
+  text_off[3 * j] = o;
+  text_off[3 * j + 1] = o + (uint64_t)(s.d - (text + o));
+  emit_old_tags(s, r);
+  text_off[3 * j + 2] = o + (uint64_t)(s.d - (text + o));
+  emit_new_tags(s, ops, r);
+  rec_out[j] = rec + global_base;
+  has_subject[j] = r.has_subj ? 1 : 0;
+}
+}  // namespace fei
+
+extern "C" int fei_corpus_tag_edit(fei_corpus* c, const uint8_t* prog, uint64_t prog_len, uint32_t op,
+                                   const uint8_t* tags, const uint64_t* tags_off, uint32_t n_tags,
+                                   uint64_t* rec, uint64_t cap, uint64_t* n_changed,
+                                   uint8_t* text, uint64_t text_cap, uint64_t* text_off, uint8_t* has_subject) {
+  if (!c || !prog || !n_changed || !text_off || (n_tags && (!tags || !tags_off))) { set_error("null argument"); return FEI_E_BADARG; }
+  if (op > 2) { set_error("unknown tag operation %u (0 add, 1 remove, 2 replace)", op); return FEI_E_BADARG; }
+  std::lock_guard<std::mutex> lock(c->mu);
+  *n_changed = 0; text_off[0] = 0;
+  const uint64_t op_bytes = n_tags ? tags_off[n_tags] - tags_off[0] : 0;
+  if (n_tags > kTagOpsMax || op_bytes > kTagBytesMax) {
+    set_error("%u tags of %llu bytes: a tag edit takes at most %u tags of %u bytes in all", n_tags, (unsigned long long)op_bytes, kTagOpsMax, kTagBytesMax);
+    return FEI_E_UNSUPPORTED;
+  }
+  TagOps ops;
+  memset(&ops, 0, sizeof(ops));
+  ops.op = op; ops.n_tags = n_tags;
+  for (uint32_t k = 0; k <= n_tags; ++k) ops.off[k] = n_tags ? (uint32_t)(tags_off[k] - tags_off[0]) : 0u;
+  if (op_bytes) memcpy(ops.bytes, tags + tags_off[0], op_bytes);
+  for (uint32_t k = 0; k < n_tags; ++k) {                        // the multiset of the operands, for replace
+    uint32_t d = 0;
+    while (d < ops.n_dist && !(ops.off[ops.dist[d] + 1] - ops.off[ops.dist[d]] == ops.off[k + 1] - ops.off[k] &&
+                               !memcmp(ops.bytes + ops.off[ops.dist[d]], ops.bytes + ops.off[k], ops.off[k + 1] - ops.off[k]))) ++d;
+    if (d == ops.n_dist) { ops.dist[d] = (uint16_t)k; ops.mult[d] = 0; ++ops.n_dist; }
+    ++ops.mult[d];
+  }
+  FEI_TRY(run_scan(c, prog, prog_len, kCompactNone, nullptr));
+  fei_prog_hdr h; memcpy(&h, prog, sizeof(h));
+  if (h.n_queries != 1 || h.n_slots < 2) { set_error("a tag edit wants one query whose first two header fields are Tags and Subject"); return FEI_E_BADARG; }
+  const uint64_t n = c->n;
+  if (n == 0) return finish_timing(c, false);
+  cudaStream_t s = ctx().stream;
+  DevBuf d_ops, d_changed, d_bytes, d_pos, d_off;
+  FEI_TRY(upload(d_ops, &ops, sizeof(ops), 0, s));
+  FEI_TRY(d_changed.alloc(n * 4)); FEI_TRY(d_bytes.alloc(n * 4)); FEI_TRY(d_pos.alloc((n + 1) * 8)); FEI_TRY(d_off.alloc((n + 1) * 8));
+  const TagEditArgs a{c->prog.as<uint8_t>(), c->hdr.as<uint8_t>(), c->hdr_off.as<uint64_t>(), c->hdir.as<uint2>(), c->hdir_off.as<uint64_t>(),
+                      c->key_lut.as<uint32_t>(), c->hits.as<uint32_t>(), n, d_ops.as<TagOps>()};
+  const unsigned grid = (unsigned)((n + 255) / 256);
+  k_tag_edit_measure<<<grid, 256, 0, s>>>(a, d_changed.as<uint32_t>(), d_bytes.as<uint32_t>());
+  FEI_TRY(exclusive_scan_u32_u64(d_changed.as<uint32_t>(), n, d_pos.as<uint64_t>(), c->scan_tmp, s));
+  FEI_TRY(exclusive_scan_u32_u64(d_bytes.as<uint32_t>(), n, d_off.as<uint64_t>(), c->scan_tmp, s));
+  uint64_t count = 0, total = 0;
+  FEI_CUDA(cudaMemcpyAsync(&count, d_pos.as<uint64_t>() + n, 8, cudaMemcpyDeviceToHost, s));
+  FEI_CUDA(cudaMemcpyAsync(&total, d_off.as<uint64_t>() + n, 8, cudaMemcpyDeviceToHost, s));
+  FEI_CUDA(cudaStreamSynchronize(s));
+  if (count > cap || total > text_cap || (count && (!rec || !text || !has_subject))) {
+    *n_changed = count; text_off[0] = total;
+    set_error("tag edit buffers too small: need %llu records and %llu text bytes", (unsigned long long)count, (unsigned long long)total);
+    return FEI_E_CAPACITY;
+  }
+  if (count) {
+    DevBuf d_rec, d_toff, d_has, d_text;
+    FEI_TRY(d_rec.alloc(count * 8)); FEI_TRY(d_toff.alloc(3 * count * 8)); FEI_TRY(d_has.alloc(count)); FEI_TRY(d_text.alloc(total + 16));
+    k_tag_edit_write<<<grid, 256, 0, s>>>(a, d_changed.as<uint32_t>(), d_pos.as<uint64_t>(), d_off.as<uint64_t>(), c->global_base,
+                                          d_rec.as<uint64_t>(), d_toff.as<uint64_t>(), d_has.as<uint8_t>(), d_text.as<uint8_t>());
+    FEI_CUDA(cudaMemcpyAsync(rec, d_rec.p, count * 8, cudaMemcpyDeviceToHost, s));
+    FEI_CUDA(cudaMemcpyAsync(text_off, d_toff.p, 3 * count * 8, cudaMemcpyDeviceToHost, s));
+    FEI_CUDA(cudaMemcpyAsync(has_subject, d_has.p, count, cudaMemcpyDeviceToHost, s));
+    if (total) FEI_CUDA(cudaMemcpyAsync(text, d_text.p, total, cudaMemcpyDeviceToHost, s));
+    FEI_CUDA(cudaStreamSynchronize(s));
+    FEI_CUDA(cudaGetLastError());
+  }
+  text_off[3 * count] = total;
+  *n_changed = count;
+  return finish_timing(c, false);
+}

@@ -10,6 +10,7 @@ replaces  memdir_tools.search.search_memories          (search.py:337)
           memdir_tools.memorychain.MemoryChain.validate_chain                (memorychain.py:596)
           memdir_tools.archiver.MemoryArchiver: archive_old_memories, cleanup_memories, empty_trash,
               apply_retention_policies, update_memory_statuses, run_maintenance   (archiver.py:205-639)
+          memdir_tools.folders.MemdirFolderManager: get_folder_stats, list_folders, bulk_tag_folder   (folders.py:216-587)
 and adds  memdir_tools.filter.apply_filters.  Names other modules already imported (`from memdir_tools.search import
 search_memories` in server.py / cli.py, the package's own re-exports) are rebound too, by identity.
 Everything else of the reference (SearchQuery objects, MemoryFilter objects, MemoryArchiver settings, block classes,
@@ -72,6 +73,27 @@ def _install_archiver(cls: Any, sync_base) -> None:
         setattr(cls, fn.__name__, fn)
 
 
+def _install_folders(cls: Any, sync_base) -> None:
+    """The folder manager's whole-folder reads run on the GPU; the manager's file-system methods stay the reference's."""
+    from .memdir_tools import folders as gfolders
+
+    def gpu() -> "gfolders.MemdirFolderManager":
+        sync_base()
+        return object.__new__(gfolders.MemdirFolderManager)      # the reference object's __init__ already made the tree
+
+    def get_folder_stats(self, folder_path, include_subfolders=False):
+        return gpu().get_folder_stats(folder_path, include_subfolders)
+
+    def list_folders(self, parent_folder="", recursive=False):
+        return gpu().list_folders(parent_folder, recursive)
+
+    def bulk_tag_folder(self, folder_path, tags, statuses=None, operation="add"):
+        return gpu().bulk_tag_folder(folder_path, tags, statuses, operation)
+
+    for fn in (get_folder_stats, list_folders, bulk_tag_folder):
+        setattr(cls, fn.__name__, fn)
+
+
 def install(package: str = "memdir_tools") -> None:
     ref_utils = importlib.import_module(f"{package}.utils")
     ref_search = importlib.import_module(f"{package}.search")
@@ -131,6 +153,12 @@ def install(package: str = "memdir_tools") -> None:
         ref_arch = None
     if ref_arch is not None:
         _install_archiver(ref_arch.MemoryArchiver, _sync_base)
+    try:
+        ref_folders = importlib.import_module(f"{package}.folders")
+    except ImportError:
+        ref_folders = None
+    if ref_folders is not None:
+        _install_folders(ref_folders.MemdirFolderManager, _sync_base)
     try:
         ref_chain = importlib.import_module(f"{package}.memorychain")
     except Exception:                                        # the reference module needs `requests`

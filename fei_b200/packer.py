@@ -423,6 +423,7 @@ class PackedMemdir:
         self._walk_cache: Optional[List[str]] = None
         self._tree_dirty = True
         self._tree_dirs: List[str] = []
+        self._dirty_dirs: set = set()                        # (folder, status) directories whose files were rewritten in place (mark_dirty)
 
     # ---- tree walk
     def _walk(self) -> List[str]:
@@ -507,8 +508,9 @@ class PackedMemdir:
                     except OSError:
                         mt = -1
                     if (seg is None or seg.mtime_ns != mt or full_check or (dirty_paths is not None and path in dirty_paths)
-                            or (isdir and not watched and now - self.last_full_check >= recheck)):
+                            or (isdir and not watched and now - self.last_full_check >= recheck) or (folder, st) in self._dirty_dirs):
                         changed.append((folder, st))
+            self._dirty_dirs.clear()
             if full_check or changed:
                 self.last_full_check = now
             if self.corpus is None:
@@ -517,6 +519,12 @@ class PackedMemdir:
                 self._set_folders(folders)
                 self._incremental(changed)
             return self
+
+    def mark_dirty(self, folder: str, status: str) -> None:
+        """Files of this directory were rewritten in place, which leaves the directory's mtime alone: the next sync lists it and
+        reads the changed files again even without inotify and before FEI_REVALIDATE_S has passed."""
+        with self.lock:
+            self._dirty_dirs.add((folder, status))
 
     def _list(self, folder: str, st: str, want_stat: bool = True) -> Tuple[DirListing, int]:
         path = self._dir(folder, st)

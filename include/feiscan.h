@@ -269,6 +269,19 @@ int fei_corpus_slot_values(fei_corpus* c, const uint8_t* prog, uint64_t prog_len
                            uint8_t* blob, uint64_t blob_cap);
 int fei_corpus_set_aux(fei_corpus* c, uint32_t k, const uint8_t* bytes, uint64_t n);
 
+/* The tag edit of MemdirFolderManager.bulk_tag_folder (memdir_tools/folders.py:483-587) over the records `prog` selects.
+ * prog: ONE query; its conditions select the records; header field 0 is the exact key "Tags" and field 1 the exact key "Subject"
+ * (give both an always-true pattern that holds when the header is absent).  op: 0 add, 1 remove, 2 replace; the operands are
+ * tags[tags_off[k] .. tags_off[k+1]), k < n_tags (at most 64 of 4096 bytes in all, else FEI_E_UNSUPPORTED).  A record is affected
+ * when the multiset of its stripped `Tags` pieces changes.  Out, per affected record j in corpus order: rec[j] its global index,
+ * has_subject[j], and three strings text[text_off[3j] .. text_off[3j+1]) = the Subject value, then ", ".join(existing), then
+ * ", ".join(updated); text_off[3 * *n_changed] = the bytes written.  FEI_E_CAPACITY when cap or text_cap is too small: then
+ * *n_changed = the affected records and text_off[0] = the text bytes needed. */
+int fei_corpus_tag_edit(fei_corpus* c, const uint8_t* prog, uint64_t prog_len, uint32_t op,
+                        const uint8_t* tags, const uint64_t* tags_off, uint32_t n_tags,
+                        uint64_t* rec, uint64_t cap, uint64_t* n_changed,
+                        uint8_t* text, uint64_t text_cap, uint64_t* text_off, uint8_t* has_subject);
+
 /* ---- Memorychain validation -----------------------------------------------------
  * Replaces the loop of MemoryChain.validate_chain (memdir_tools/memorychain.py:596-618)
  * and its inline copy in receive_chain_update (:1059-1078):
