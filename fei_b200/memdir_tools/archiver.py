@@ -35,10 +35,13 @@ def compile_criteria(criteria: Dict[str, Any], now: datetime) -> List[List[List[
             if isinstance(pattern, bool) or not isinstance(pattern, int):
                 raise NotImplementedError(f"criteria {key!r}: only integer day counts are supported on the GPU")
             # (now - date).days < p  <=>  date > now - p days;  .days > p  <=>  date <= now - (p + 1) days   (timedelta.days floors)
-            if key in ("age", "min_age"):
-                out.append([[Cond(C_DATE_CMP, op=CMP["<="], i64=_micros(now - timedelta(days=pattern)))]])
-            else:
-                out.append([[Cond(C_DATE_CMP, op=CMP[">"], i64=_micros(now - timedelta(days=pattern + 1)))]])
+            days = pattern if key in ("age", "min_age") else pattern + 1
+            try:
+                edge = _micros(now - timedelta(days=days))
+            except OverflowError:                              # the edge lies outside datetime's years 1..9999: every date is on one side
+                out.append([[const((key == "max_age") == (days > 0))]])
+                continue
+            out.append([[Cond(C_DATE_CMP, op=CMP["<="] if key in ("age", "min_age") else CMP[">"], i64=edge)]])
         elif key in ("tag", "tags"):
             items = pattern if isinstance(pattern, list) else [pattern.lower()]
             alts = []

@@ -114,11 +114,17 @@ def parse_search_args(args_str: str) -> SearchQuery:
 
 # ----------------------------------------------------------------------------- query compiler
 class _Raises:
-    """A condition that raises in the reference for every record that reaches it with a non-None value."""
+    """A condition that raises in the reference for every record that reaches it and satisfies `presence` (every record that
+    reaches it when `presence` is None).  The records it does not raise for go on to the next item of the compiled list."""
 
     def __init__(self, exc: Exception, presence: Optional[Cond], exc_of=None):
         self.exc, self.presence = exc, presence
         self.exc_of = exc_of                 # record index -> the exception that record raises (when the records differ in that)
+
+
+def _type_name(v: Any) -> str:
+    """The type name Python's comparison TypeError shows: the C type's tp_name, so datetime is 'datetime.datetime'."""
+    return "datetime.datetime" if isinstance(v, datetime) else type(v).__name__
 
 
 def _string_pattern(op: str, v2: Any, v1_name: str):
@@ -146,7 +152,7 @@ def _string_pattern(op: str, v2: Any, v1_name: str):
             if v2 == "now" or (v2.startswith("now") and re.match(r"now([+-])(\d+)([dwmy])", v2)):
                 return TypeError(f"'{op}' not supported between instances of 'str' and 'datetime.datetime'"), False
             return Pattern({">": "cmp_gt", "<": "cmp_lt", ">=": "cmp_ge", "<=": "cmp_le"}[op], v2), False
-        return TypeError(f"'{op}' not supported between instances of 'str' and '{type(v2).__name__}'"), False
+        return TypeError(f"'{op}' not supported between instances of 'str' and '{_type_name(v2)}'"), False
     if op == "has_flag":
         return Pattern("exact_contains", str(v2).upper()), False
     return False, False                                    # unknown operator
@@ -181,7 +187,7 @@ def _slot(field: str, mode: int, empty: bool, pat, neg, if_missing: int = 0) -> 
         # constant verdict, but a missing header (None) is always False (search.py:144-145)
         return [present if pat else const(False)] if not empty else [const(pat)]
     if isinstance(pat, Exception):
-        return [_Raises(pat, None if empty else present)]
+        return [_Raises(pat, None)] if empty else [_Raises(pat, present), const(False)]     # no header: None, which is False
     return [Cond(C_SLOT, pattern=pat, negate=neg, field=field, mode=mode, empty_if_missing=empty, if_missing=if_missing)]
 
 
@@ -249,8 +255,10 @@ def _compile_date(op: str, v2: Any) -> List[Any]:
     if not isinstance(v2, datetime):
         try:
             v2 = dateutil.parser.parse(str(v2))
-        except (ValueError, TypeError, OverflowError):
+        except (ValueError, TypeError):
             return [const(False)]
+        except OverflowError as e:                       # not caught by the reference: the first record that reaches it raises
+            return [_Raises(e, None)]
     if v2.tzinfo is not None and v2.utcoffset() is not None:
         if op == "=":
             return [const(False)]                        # naive == aware is False, != is True
@@ -285,7 +293,7 @@ def _int_cmp_cond(op: str, v2: Any) -> List[Any]:
     if not isinstance(v2, int):
         if op in ("=", "!="):
             return [const(op == "!=")]                    # int == <other object> is False
-        return [_Raises(TypeError(f"'{op}' not supported between instances of 'int' and '{type(v2).__name__}'"), None)]
+        return [_Raises(TypeError(f"'{op}' not supported between instances of 'int' and '{_type_name(v2)}'"), None)]
     big = (1 << 63) - 1
     if v2 > big or v2 < -big:
         return [const({">": v2 < 0, ">=": v2 < 0, "<": v2 > 0, "<=": v2 > 0, "=": False, "!=": True}[op])]
@@ -325,25 +333,29 @@ def _compile_timestamp(field: str, op: str, v2: Any, pm) -> List[Any]:
             return meta
         present = Cond(C_SLOT, pattern=Pattern("regex", "", re.IGNORECASE), negate=(op == "="), field=field, mode=0, if_missing=2)
         return [present] + meta if not isinstance(meta[0], _Raises) else meta
-    exc = TypeError(f"'{op}' not supported between instances of 'str' and '{type(v2).__name__}'")
+    exc = TypeError(f"'{op}' not supported between instances of 'str' and '{_type_name(v2)}'")
     present = Cond(C_SLOT, pattern=Pattern("regex", "", re.IGNORECASE), field=field, mode=0)
     return [_Raises(exc, present)] + meta
 
 
 def _parse_dt(value: str):
     """dateutil.parser.parse as search.py:126-130 calls it, plus whether the result depends on today's date (missing
-    fields are taken from `default` = today): such values must be parsed again for every query."""
+    fields are taken from `default` = today): such values must be parsed again for every query.  A value dateutil overflows
+    on gives the OverflowError: the reference does not catch it, so reading that value raises, whatever the operator."""
     try:
         a = dateutil.parser.parse(value, default=datetime(2001, 1, 1))
         b = dateutil.parser.parse(value, default=datetime(2002, 2, 2))
-    except (ValueError, TypeError, OverflowError):
+    except (ValueError, TypeError):
         return None, False
+    except OverflowError as e:
+        return e, False
     return a, a != b
 
 
 def _judge_value(v1: Any, op: str, v2: Any) -> bool:
     """The reference's comparison of ONE resolved field value with the operand (search.py:141-242), applied on the host to
-    the distinct values of a date-like header (a datetime when dateutil could parse it, else the raw string).  May raise TypeError."""
+    the distinct values of a date-like header (a datetime when dateutil could parse it, else the raw string).  May raise TypeError,
+    or OverflowError when dateutil overflows on the operand."""
     if op == "contains":
         return str(v2).lower() in str(v1).lower()
     if op == "matches":
@@ -396,11 +408,16 @@ def _compile_date_header(field: str, op: str, v2: Any, pm) -> List[Any]:
         if parsed is None:
             parsed = pm.parsed_dates[text] = _parse_dt(text)
         dt, today_dependent = parsed
+        if isinstance(dt, OverflowError):
+            bad[k] = 1
+            excs[k] = OverflowError(*dt.args)
+            first_exc = first_exc or excs[k]
+            continue
         if today_dependent:
             dt = dateutil.parser.parse(text)
         try:
             ok[k] = 1 if _judge_value(dt if dt is not None else text, op, v2) else 0
-        except TypeError as e:
+        except (TypeError, OverflowError) as e:
             bad[k] = 1
             excs[k] = e
             first_exc = first_exc or e
@@ -422,6 +439,16 @@ def _scan_ranges(pm, conds: List[Cond], ranges: List[Tuple[int, int]]) -> np.nda
         lo, hi = np.searchsorted(hits, a), np.searchsorted(hits, b)
         parts.append(hits[lo:hi])
     return np.concatenate(parts) if parts else np.zeros(0, dtype=np.int64)
+
+
+def _listing_position(ranges: List[Tuple[int, int]], i: int) -> int:
+    """Position of packed record i in the listing the requested segments make."""
+    pos = 0
+    for a, b in ranges:
+        if a <= i < b:
+            return pos + i - a
+        pos += b - a
+    raise ValueError(i)
 
 
 def _get_field_value(memory: Dict[str, Any], field: str) -> Any:
@@ -465,16 +492,24 @@ def search_memories(query: SearchQuery, folders: Optional[List[str]] = None, sta
         pm.begin_query()
         compiled = compile_conditions(query.conditions, query.include_content, pm)
         conds: List[Cond] = []
+        first: Optional[Tuple[int, Exception]] = None     # (listing position, exception) of the first record the reference raises at
         for item in compiled:
             if isinstance(item, _Raises):
-                # the reference raises as soon as one record reaches this condition with a value
+                # the reference raises at the first record (in listing order) that reaches a raising condition
                 probe = conds + ([item.presence] if item.presence is not None else [])
                 reached = _scan_ranges(pm, probe or [const(True)], ranges)
                 if len(reached):
-                    raise (item.exc_of(int(reached[0])) if item.exc_of else item.exc)
-                conds.append(const(False))               # nobody reaches it: everything was rejected earlier
-                break
+                    i = int(reached[0])
+                    pos = _listing_position(ranges, i)
+                    if first is None or pos < first[0]:
+                        first = (pos, item.exc_of(i) if item.exc_of else item.exc)
+                if item.presence is None:
+                    conds.append(const(False))           # every record that reaches it raises: none goes further
+                    break
+                continue
             conds.append(item)
+        if first is not None:
+            raise first[1]
         hits = _scan_ranges(pm, conds or [const(True)], ranges)
         results = pm.materialize(hits, query.include_content)
     if query.sort_by:
