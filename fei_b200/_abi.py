@@ -17,6 +17,8 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libfeiscan.so")
 
 FEI_OK, FEI_E_CUDA, FEI_E_NCCL, FEI_E_CAPACITY, FEI_E_UNSUPPORTED, FEI_E_BADARG, FEI_E_STATE = 0, -1, -2, -3, -4, -5, -6
+FEI_FMT_JSON, FEI_FMT_CSV, FEI_FMT_COMPACT, FEI_FMT_TEXT = 0, 1, 2, 3            # fei_corpus_format_records
+FEI_FMT_CONTENT, FEI_FMT_SEPARATOR = 0x1, 0x2
 NCCL_ID_BYTES = 128
 CHAIN_NCOLS = 10
 J_NULL, J_STR, J_INT, J_FLOAT, J_TRUE, J_FALSE, J_BIGINT = range(7)
@@ -113,6 +115,7 @@ _SIGS = {
     "fei_corpus_slot_values": (C.c_int, [_P, _P, _U64, _P, _P, _P, _U64]),
     "fei_corpus_set_aux": (C.c_int, [_P, C.c_uint32, _P, _U64]),
     "fei_corpus_tag_edit": (C.c_int, [_P, _P, _U64, C.c_uint32, _P, _P, C.c_uint32, _P, _U64, _P, _P, _U64, _P, _P]),
+    "fei_corpus_format_records": (C.c_int, [_P, _P, _U64, C.c_uint32, C.c_uint32, _P, _P, C.c_uint32, _P, _U64, _P, _P]),
     "fei_chain_validate_msgs": (C.c_int, [_P, _P, _P, _P, _P, _P, _U64, _U64, _P, _P, _P]),
     "fei_chain_validate_cols": (C.c_int, [_P, _P, _P, _U64, _U64, _P, _P, _P, _P, _U64, _P]),
     "fei_chain_create": (C.c_int, [_P]),

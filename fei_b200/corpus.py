@@ -211,6 +211,33 @@ class Corpus:
         out = [(raw[o[3 * j]:o[3 * j + 1]] if has[j] else None, raw[o[3 * j + 1]:o[3 * j + 2]], raw[o[3 * j + 2]:o[3 * j + 3]]) for j in range(k)]
         return rec[:k].copy(), out
 
+    def format_records(self, idx: np.ndarray, fmt: int, opts: int, folder_names: Sequence[bytes], cap: Optional[int] = None):
+        """What the command line prints for records idx (corpus-local, output order), written on the GPU (fei_corpus_format_records,
+        formats _abi.FEI_FMT_*): (bytes, offsets[m+1]).  With `cap`, at most that many bytes: when the records need more, returns
+        (None, offsets) so the caller can take a prefix that fits."""
+        idx = np.ascontiguousarray(idx, dtype=np.uint64)
+        m = idx.size
+        names = b"".join(folder_names)
+        fblob = np.frombuffer(names, dtype=np.uint8) if names else np.zeros(1, dtype=np.uint8)
+        foff = np.zeros(len(folder_names) + 1, dtype=np.uint64)
+        foff[1:] = np.cumsum([len(f) for f in folder_names], dtype=np.uint64)
+        off = np.zeros(m + 1, dtype=np.uint64)
+        l = _abi.lib()
+        ms = C.c_float()
+        size = cap if cap is not None else 0
+        while True:
+            out = np.empty(max(1, size), dtype=np.uint8)
+            rc = l.fei_corpus_format_records(self._h, _abi.ptr(idx), m, fmt, opts, _abi.ptr(fblob), _abi.ptr(foff), len(folder_names),
+                                             _abi.ptr(out), size, _abi.ptr(off), C.byref(ms))
+            if rc != _abi.FEI_E_CAPACITY or cap is not None:
+                break
+            size = int(off[m])                                      # sized by the failed call: the retry fits
+        self.last_format_ms = float(ms.value)
+        if rc == _abi.FEI_E_CAPACITY:
+            return None, off
+        _abi.check(rc)
+        return out[:int(off[m])].tobytes(), off
+
     def set_aux(self, k: int, verdicts: Optional[np.ndarray]) -> None:
         """Aux column k: one host-computed verdict byte per record, read by C_RECBITS conditions (fei_corpus_set_aux)."""
         if verdicts is None:

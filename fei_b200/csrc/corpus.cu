@@ -161,6 +161,22 @@ static int fetch_bodies(fei_corpus* c, const uint64_t* d_idx, uint64_t first, ui
   return FEI_OK;
 }
 
+int untile_bodies(fei_corpus* c, const uint64_t* d_idx, uint64_t m, DevBuf& d_boff, DevBuf& d_body, cudaStream_t s) {
+  DevBuf d_hlen, d_blen;
+  FEI_TRY(d_hlen.alloc(m * 4 + 4)); FEI_TRY(d_blen.alloc(m * 4 + 4)); FEI_TRY(d_boff.alloc((m + 1) * 8));
+  if (m) k_rec_lens<<<(unsigned)((m + 127) / 128), 128, 0, s>>>(d_idx, 0, m, c->hdr_off.as<uint64_t>(), c->rec_pos.as<uint32_t>(), c->grp_len.as<uint32_t>(),
+                                                                d_hlen.as<uint32_t>(), d_blen.as<uint32_t>());
+  FEI_TRY(exclusive_scan_u32_u64(d_blen.as<uint32_t>(), m, d_boff.as<uint64_t>(), c->scan_tmp, s));
+  uint64_t total = 0;
+  FEI_CUDA(cudaMemcpyAsync(&total, d_boff.as<uint64_t>() + m, 8, cudaMemcpyDeviceToHost, s));
+  FEI_CUDA(cudaStreamSynchronize(s));
+  FEI_TRY(d_body.alloc(total + 16));
+  if (m) k_untile_idx<<<(unsigned)((m + 127) / 128), 128, 0, s>>>(c->tiles.as<uint8_t>(), c->grp_base.as<uint64_t>(), c->grp_len.as<uint32_t>(), c->rec_pos.as<uint32_t>(),
+                                                                  d_idx, 0, m, d_boff.as<uint64_t>(), d_body.as<uint8_t>());
+  FEI_CUDA(cudaGetLastError());
+  return FEI_OK;
+}
+
 int corpus_load_events(fei_corpus* c) {
   for (auto& e : c->ev_load) if (!e) FEI_CUDA(cudaEventCreate(&e));
   return FEI_OK;

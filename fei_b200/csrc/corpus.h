@@ -112,6 +112,9 @@ int pack_canonical(fei_corpus* c, DevBuf& body, DevBuf& body_off, cudaStream_t s
 // builds the header directory from hdr / hdr_off already on the device (hdir.cu)
 int build_header_dir(fei_corpus* c, cudaStream_t s);
 int exclusive_scan_u32_u64(const uint32_t* in, uint64_t n, uint64_t* out, DevBuf& tmp, cudaStream_t s);
+// The bodies of records d_idx[0..m) (device array) un-tiled on the device: d_boff gets their m + 1 offsets, d_body the bytes
+// (k_rec_lens, a scan and k_untile_idx, queued on s after one wait for the total).
+int untile_bodies(fei_corpus* c, const uint64_t* d_idx, uint64_t m, DevBuf& d_boff, DevBuf& d_body, cudaStream_t s);
 // Multi-GPU exchange of a scan (comm.cu).
 struct ScanHook {
   // if set, the scan kernel itself stores every finished window's hit masks into these peer buffers (device array of push_n

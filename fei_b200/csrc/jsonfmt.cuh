@@ -10,7 +10,7 @@
 
 #if defined(__CUDACC__)
 #define FEI_JHD __host__ __device__ __forceinline__
-#define FEI_JHD_NI __host__ __device__
+#define FEI_JHD_NI __host__ __device__ inline
 #else
 #define FEI_JHD inline
 #define FEI_JHD_NI inline
@@ -205,6 +205,21 @@ template <class S> FEI_JHD void put_u4(S& o, uint32_t cp) {      // \uXXXX, lowe
   o.put('\\'); o.put('u'); o.put((uint8_t)hx[(cp >> 12) & 15]); o.put((uint8_t)hx[(cp >> 8) & 15]); o.put((uint8_t)hx[(cp >> 4) & 15]); o.put((uint8_t)hx[cp & 15]);
 }
 
+// one ASCII character as py_encode_basestring_ascii writes it (put_json_string keeps its own copy of this switch: routing it
+// through here changes the SASS of the chain kernels that instantiate it)
+template <class S> FEI_JHD void put_json_ascii(S& o, uint32_t c) {
+  switch (c) {
+    case '"': o.put('\\'); o.put('"'); break;
+    case '\\': o.put('\\'); o.put('\\'); break;
+    case '\n': o.put('\\'); o.put('n'); break;
+    case '\r': o.put('\\'); o.put('r'); break;
+    case '\t': o.put('\\'); o.put('t'); break;
+    case '\b': o.put('\\'); o.put('b'); break;
+    case '\f': o.put('\\'); o.put('f'); break;
+    default: if (c >= 0x20 && c <= 0x7E) o.put((uint8_t)c); else put_u4(o, c);
+  }
+}
+
 // py_encode_basestring_ascii: everything outside ' '..'~' plus '"' and '\\' is escaped.  Input is UTF-8 (lone surrogates
 // arrive as 3-byte "surrogatepass" sequences).
 template <class S> FEI_JHD_NI void put_json_string(S& o, const uint8_t* s, uint64_t n) {
@@ -231,6 +246,41 @@ template <class S> FEI_JHD_NI void put_json_string(S& o, const uint8_t* s, uint6
     else if ((c & 0xF0) == 0xE0) { cp = c & 0x0F; len = 3; }
     else { cp = c & 0x07; len = 4; }
     for (int k = 1; k < len && i + k < n; ++k) cp = (cp << 6) | (s[i + k] & 0x3F);
+    i += len;
+    if (cp >= 0x10000) { const uint32_t v = cp - 0x10000; put_u4(o, 0xD800 | (v >> 10)); put_u4(o, 0xDC00 | (v & 0x3FF)); }
+    else put_u4(o, cp);
+  }
+  o.put('"');
+}
+
+// Length of the well-formed UTF-8 sequence at s[0..n) (Python's strict decoder: no overlongs, surrogates or code points past
+// U+10FFFF), or 0 when s[0] does not start one.
+FEI_JHD uint32_t utf8_seq_len(const uint8_t* s, uint64_t n) {
+  const uint32_t c = s[0];
+  if (c < 0x80) return 1;
+  uint32_t len, lo = 0x80, hi = 0xBF;
+  if (c >= 0xC2 && c <= 0xDF) len = 2;
+  else if (c >= 0xE0 && c <= 0xEF) { len = 3; if (c == 0xE0) lo = 0xA0; if (c == 0xED) hi = 0x9F; }
+  else if (c >= 0xF0 && c <= 0xF4) { len = 4; if (c == 0xF0) lo = 0x90; if (c == 0xF4) hi = 0x8F; }
+  else return 0;
+  if (n < len || s[1] < lo || s[1] > hi) return 0;
+  for (uint32_t k = 2; k < len; ++k) if ((s[k] & 0xC0) != 0x80) return 0;
+  return len;
+}
+
+// put_json_string of a file-system name as os.fsdecode gives it: bytes that are not part of well-formed UTF-8 become the lone
+// surrogates U+DC80..U+DCFF (surrogateescape), which json.dumps writes as \udcXX.
+template <class S> FEI_JHD void put_json_fsname(S& o, const uint8_t* s, uint64_t n) {
+  o.put('"');
+  for (uint64_t i = 0; i < n;) {
+    const uint32_t len = utf8_seq_len(s + i, n - i);
+    if (len == 0) { put_u4(o, 0xDC00u | s[i]); ++i; continue; }
+    if (len == 1) {                                                  // ASCII: the escapes of put_json_string
+      put_json_ascii(o, s[i++]);
+      continue;
+    }
+    uint32_t cp = s[i] & (0x7Fu >> len);
+    for (uint32_t k = 1; k < len; ++k) cp = (cp << 6) | (s[i + k] & 0x3F);
     i += len;
     if (cp >= 0x10000) { const uint32_t v = cp - 0x10000; put_u4(o, 0xD800 | (v >> 10)); put_u4(o, 0xDC00 | (v & 0x3FF)); }
     else put_u4(o, cp);

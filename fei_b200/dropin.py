@@ -11,6 +11,8 @@ replaces  memdir_tools.search.search_memories          (search.py:337)
           memdir_tools.archiver.MemoryArchiver: archive_old_memories, cleanup_memories, empty_trash,
               apply_retention_policies, update_memory_statuses, run_maintenance   (archiver.py:205-639)
           memdir_tools.folders.MemdirFolderManager: get_folder_stats, list_folders, bulk_tag_folder   (folders.py:216-587)
+          memdir_tools.cli: list_memories_cmd, view_memory, move_memory_cmd, search_memories_cmd, flag_memory   (cli.py:103-268)
+          memdir_tools.search.main                      (search.py:596, what `python -m memdir_tools search` calls)
 and adds  memdir_tools.filter.apply_filters.  Names other modules already imported (`from memdir_tools.search import
 search_memories` in server.py / cli.py, the package's own re-exports) are rebound too, by identity.
 Everything else of the reference (SearchQuery objects, MemoryFilter objects, MemoryArchiver settings, block classes,
@@ -94,6 +96,19 @@ def _install_folders(cls: Any, sync_base) -> None:
         setattr(cls, fn.__name__, fn)
 
 
+def _install_functions(ref_mod: Any, gpu_mod: Any, names, sync_base) -> None:
+    """Module-level functions of the reference that run their GPU namesake against the reference's tree."""
+    for name in names:
+        fn = getattr(gpu_mod, name)
+
+        def run(*a, _fn=fn, **k):
+            sync_base()
+            return _fn(*a, **k)
+        run.__name__ = run.__qualname__ = name
+        _rebind(getattr(ref_mod, name), run)
+        setattr(ref_mod, name, run)
+
+
 def install(package: str = "memdir_tools") -> None:
     ref_utils = importlib.import_module(f"{package}.utils")
     ref_search = importlib.import_module(f"{package}.search")
@@ -159,6 +174,16 @@ def install(package: str = "memdir_tools") -> None:
         ref_folders = None
     if ref_folders is not None:
         _install_folders(ref_folders.MemdirFolderManager, _sync_base)
+    try:
+        ref_cli = importlib.import_module(f"{package}.cli")
+    except ImportError:
+        ref_cli = None
+    if ref_cli is not None:                                 # the command line's listing, lookup and search commands; create / mkdir stay
+        from .memdir_tools import cli as gcli
+        _install_functions(ref_cli, gcli, ("list_memories_cmd", "view_memory", "move_memory_cmd", "search_memories_cmd", "flag_memory"),
+                           _sync_base)
+    if hasattr(ref_search, "main"):
+        _install_functions(ref_search, gsearch, ("main",), _sync_base)
     try:
         ref_chain = importlib.import_module(f"{package}.memorychain")
     except Exception:                                        # the reference module needs `requests`

@@ -483,9 +483,11 @@ def _get_field_value(memory: Dict[str, Any], field: str) -> Any:
     return None
 
 
-def search_memories(query: SearchQuery, folders: Optional[List[str]] = None, statuses: Optional[List[str]] = None,
-                    debug: bool = False) -> List[Dict[str, Any]]:
-    pm = packer.packed()
+def search_positions(pm: "packer.PackedMemdir", query: SearchQuery, folders: Optional[List[str]] = None,
+                     statuses: Optional[List[str]] = None) -> Tuple[np.ndarray, Optional[List[Dict[str, Any]]]]:
+    """The hits of search_memories as listing positions of the packed tree `pm`, in the order search_memories returns them (sorted
+    and paginated).  When the query sorts, the sort runs on the materialised dicts as in the reference; those dicts come back too
+    (with content when the query includes it), else None.  The caller holds `pm.lock` while it uses the positions."""
     with pm.lock:                                        # one snapshot of the packed corpus (and its aux columns) for the whole request
         ranges = pm.ranges(folders, statuses)
         pm.report_skipped(folders, statuses)
@@ -511,15 +513,103 @@ def search_memories(query: SearchQuery, folders: Optional[List[str]] = None, sta
         if first is not None:
             raise first[1]
         hits = _scan_ranges(pm, conds or [const(True)], ranges)
-        results = pm.materialize(hits, query.include_content)
-    if query.sort_by:
-        try:
-            results.sort(key=lambda x: _get_field_value(x, query.sort_by) or "", reverse=query.sort_reverse)
-        except Exception as e:
-            print(f"Warning: Unable to sort results: {e}")
-            results.sort(key=lambda x: x["metadata"]["timestamp"], reverse=True)
-    if query.offset or query.limit:
-        start = query.offset
-        end = None if query.limit is None else start + query.limit
-        results = results[start:end]
-    return results
+        results = None
+        if query.sort_by:
+            pairs = list(zip(hits.tolist(), pm.materialize(hits, query.include_content)))
+            try:
+                pairs.sort(key=lambda x: _get_field_value(x[1], query.sort_by) or "", reverse=query.sort_reverse)
+            except Exception as e:
+                print(f"Warning: Unable to sort results: {e}")
+                pairs.sort(key=lambda x: x[1]["metadata"]["timestamp"], reverse=True)
+            hits = np.array([p for p, _ in pairs], dtype=np.int64)
+            results = [m for _, m in pairs]
+        if query.offset or query.limit:
+            start = query.offset
+            end = None if query.limit is None else start + query.limit
+            hits = hits[start:end]
+            results = results[start:end] if results is not None else None
+    return hits, results
+
+
+def search_memories(query: SearchQuery, folders: Optional[List[str]] = None, statuses: Optional[List[str]] = None,
+                    debug: bool = False) -> List[Dict[str, Any]]:
+    pm = packer.packed()
+    with pm.lock:
+        hits, results = search_positions(pm, query, folders, statuses)
+        return results if results is not None else pm.materialize(hits, query.include_content)
+
+
+def main() -> None:
+    """The search command line (search.py:596-751): the query from the positional words and the filter options, results printed
+    by print_search_results' formats from bytes the GPU writes.  --debug prints the query summary; the per-record trace of
+    search_memories(debug=True) is not reproduced."""
+    import argparse
+    from .cli import print_results
+    parser = argparse.ArgumentParser(description="Search memories on the GPU (query syntax of parse_search_args)")
+    parser.add_argument("query", nargs="*", help="Query words, field operators and shortcuts")
+    parser.add_argument("-f", "--folder", help="Folder (default: all)")
+    parser.add_argument("-s", "--status", choices=STANDARD_FOLDERS, help="Status directory (default: all)")
+    parser.add_argument("--subject", help="Subject contains")
+    parser.add_argument("--content", help="Content contains")
+    parser.add_argument("--tags", help="Tags to have (comma-separated)")
+    parser.add_argument("--priority", choices=["high", "medium", "low"], help="Priority equals")
+    parser.add_argument("--status-filter", help="Status header equals")
+    parser.add_argument("--date-from", help="Date header at or after")
+    parser.add_argument("--date-to", help="Date header at or before")
+    parser.add_argument("--flags", help="Flag letters to have")
+    parser.add_argument("--format", choices=["text", "json", "csv", "compact"], default="text", help="Output format")
+    parser.add_argument("--sort", help="Sort field")
+    parser.add_argument("--reverse", action="store_true", help="Reverse the sort")
+    parser.add_argument("--limit", type=int, help="At most this many results")
+    parser.add_argument("--offset", type=int, default=0, help="Skip this many results")
+    parser.add_argument("--with-content", action="store_true", help="Include the content")
+    parser.add_argument("--debug", action="store_true", help="Print the query first")
+    args = parser.parse_args()
+    query = SearchQuery()
+    if args.subject:
+        query.add_condition("Subject", "contains", args.subject)
+    if args.content:
+        query.add_condition("content", "contains", args.content)
+    if args.tags:
+        for tag in args.tags.split(","):
+            query.add_condition("Tags", "has_tag", tag.strip())
+    if args.priority:
+        query.add_condition("Priority", "=", args.priority)
+    if args.status_filter:
+        query.add_condition("Status", "=", args.status_filter)
+    if args.date_from:
+        query.add_condition("Date", ">=", args.date_from)
+    if args.date_to:
+        query.add_condition("Date", "<=", args.date_to)
+    if args.flags:
+        for flag in args.flags:
+            query.add_condition("flags", "has_flag", flag)
+    if args.sort:
+        query.set_sort(args.sort, args.reverse)
+    query.set_pagination(args.limit, args.offset)
+    query.with_content(args.with_content)
+    if args.query:
+        parsed = parse_search_args(" ".join(args.query))
+        query.conditions.extend(parsed.conditions)
+        if args.sort is None and parsed.sort_by:
+            query.sort_by, query.sort_reverse = parsed.sort_by, parsed.sort_reverse
+        if args.limit is None and parsed.limit:
+            query.limit = parsed.limit
+        if not args.with_content and parsed.include_content:
+            query.include_content = True
+    folders = [args.folder] if args.folder else None
+    statuses = [args.status] if args.status else None
+    if args.debug:
+        print("Search query:")
+        for c in query.conditions:
+            print(f"  - {c['field']} {c['operator']} {c['value']}")
+        print(f"Sort by: {query.sort_by or 'None'} {'(reverse)' if query.sort_reverse else ''}")
+        print(f"Limit: {query.limit or 'None'}, Offset: {query.offset}")
+        print(f"Include content: {query.include_content}")
+        print(f"Folders: {folders or 'All'}")
+        print(f"Statuses: {statuses or 'All'}")
+        print("")
+    pm = packer.packed()
+    with pm.lock:
+        hits, _ = search_positions(pm, query, folders, statuses)
+        print_results(pm, hits, args.format, query.include_content)

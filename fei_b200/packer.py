@@ -31,7 +31,7 @@ import struct
 import threading
 import time
 from datetime import datetime
-from typing import Any, Dict, List, Optional, Sequence, Tuple
+from typing import Any, Dict, Iterator, List, Optional, Sequence, Tuple
 
 import numpy as np
 
@@ -44,6 +44,7 @@ MAX_BODY = 32 << 20                                                # packed layo
 MAX_RAW_BATCH = 40 << 30                                           # raw bytes packed in one go
 COLD_CHUNK_BYTES = 256 << 20                                        # cold pack: bytes per host chunk
 COLD_SLOTS = 3                                                      # reused chunk buffers (one being read into, up to two being uploaded)
+FORMAT_CHUNK_BYTES = 64 << 20                                      # formatted output held at once (PackedMemdir.format_records)
 LIST_CONCURRENCY = 4                                                # directories listed at the same time in a cold pack
 READ_THREADS = max(1, min(32, len(os.sched_getaffinity(0)) if hasattr(os, "sched_getaffinity") else (os.cpu_count() or 1)))
 _KEY_DT = np.dtype([("ino", "u8"), ("size", "u8"), ("mtime", "i8")])
@@ -1190,6 +1191,36 @@ class PackedMemdir:
                     mem["content"] = body_text[j]
                 out[j] = mem
         return out  # type: ignore[return-value]
+
+    def format_records(self, positions: Sequence[int], fmt: int, opts: int) -> Iterator[Tuple[bytes, np.ndarray]]:
+        """What the command line prints for the records at these listing positions, in their order (Corpus.format_records: the GPU
+        writes every record's bytes), as (bytes, offsets) chunks: record k of a chunk is bytes[offsets[k]:offsets[k + 1]].  Consecutive
+        positions of the same corpus (base or delta) go to one device call; a chunk holds at most FORMAT_CHUNK_BYTES (or one record,
+        when a record alone is larger)."""
+        positions = np.asarray(positions, dtype=np.int64)
+        if not len(positions):
+            return
+        dev = self.dev[positions]
+        names = [b""] * len(self.folder_ids)
+        for f, k in self.folder_ids.items():
+            names[k] = os.fsencode(f)
+        in_delta = (dev >= self.n_base).astype(np.int8)
+        cuts = [0] + (np.nonzero(np.diff(in_delta))[0] + 1).tolist() + [len(dev)]
+        budget = FORMAT_CHUNK_BYTES
+        for a, b in zip(cuts[:-1], cuts[1:]):
+            corpus, lo = (self.delta, self.n_base) if in_delta[a] else (self.corpus, 0)
+            local = dev[a:b] - lo
+            k, step = 0, 4096
+            while k < len(local):
+                take = local[k:k + step]
+                data, off = corpus.format_records(take, fmt, opts, names, cap=budget)
+                if data is None:                                       # too many bytes: the prefix that fits (at least one record)
+                    fit = max(1, int(np.searchsorted(off, budget, side="right")) - 1)
+                    take = take[:fit]
+                    data, off = corpus.format_records(take, fmt, opts, names, cap=int(off[fit]))
+                yield data, off
+                k += len(take)
+                step = max(1, min(1 << 20, int(budget // max(1, int(off[-1]) // len(take)))))
 
     # ---- per-record header values for conditions only Python can judge (search.py:126-130)
     def header_values(self, field: str) -> Tuple[np.ndarray, np.ndarray, List[str]]:

@@ -282,6 +282,24 @@ int fei_corpus_tag_edit(fei_corpus* c, const uint8_t* prog, uint64_t prog_len, u
                         uint64_t* rec, uint64_t cap, uint64_t* n_changed,
                         uint8_t* text, uint64_t text_cap, uint64_t* text_off, uint8_t* has_subject);
 
+/* What the Memdir command line prints for the records idx[0..m) (corpus-local, any order, repeats allowed), written on the GPU
+ * from the packed corpus for the dict list_memories builds (memdir_tools/utils.py:202-253):
+ *   FEI_FMT_JSON     one element of json.dumps(results, indent=2), "  {" .. "  }" (cli.py:117-121, search.py:533-552); the caller
+ *                    adds "[\n", ",\n" and "\n]".  FEI_FMT_CONTENT adds the "content" key.
+ *   FEI_FMT_CSV      one row of the csv output, with its '\n' (search.py:554-571)
+ *   FEI_FMT_COMPACT  one line of the compact output, with its '\n' (search.py:573-582)
+ *   FEI_FMT_TEXT     print_memory (cli.py:41-67) with the content section when FEI_FMT_CONTENT is set; FEI_FMT_SEPARATOR appends
+ *                    the "-" * 34 line the search commands print after each record
+ * folder_names[folder_off[k] .. folder_off[k+1]) = memory["folder"] of packed folder id k (k < n_folders).  Record i's bytes are
+ * out[out_off[i] .. out_off[i+1]); out_off (m + 1 entries) is filled even when out is NULL or shorter than out_off[m], which
+ * returns FEI_E_CAPACITY.  kernel_ms (may be NULL) = device time of the call (CUDA events: body gather, both passes).      */
+enum { FEI_FMT_JSON = 0, FEI_FMT_CSV = 1, FEI_FMT_COMPACT = 2, FEI_FMT_TEXT = 3 };
+#define FEI_FMT_CONTENT   0x1u
+#define FEI_FMT_SEPARATOR 0x2u
+int fei_corpus_format_records(fei_corpus* c, const uint64_t* idx, uint64_t m, uint32_t fmt, uint32_t opts,
+                              const uint8_t* folder_names, const uint64_t* folder_off, uint32_t n_folders,
+                              uint8_t* out, uint64_t out_cap, uint64_t* out_off, float* kernel_ms);
+
 /* ---- Memorychain validation -----------------------------------------------------
  * Replaces the loop of MemoryChain.validate_chain (memdir_tools/memorychain.py:596-618)
  * and its inline copy in receive_chain_update (:1059-1078):
