@@ -245,75 +245,6 @@ struct fei_chain {
 
 namespace fei {
 
-// Simple three-phase exclusive scan of u32 -> u64 (n up to 2^40): per-block sums,
-// serial scan of the block sums by one thread block, then per-block rescan.
-constexpr int kScanBlock = 1024;
-__global__ void k_scan_block_sums(const uint32_t* __restrict__ in, uint64_t n, uint64_t* __restrict__ sums) {
-  __shared__ uint64_t sh[32];
-  uint64_t i = blockIdx.x * (uint64_t)kScanBlock + threadIdx.x;
-  uint64_t v = i < n ? in[i] : 0;
-  for (int o = 16; o; o >>= 1) v += __shfl_down_sync(0xffffffffu, v, o);
-  if ((threadIdx.x & 31) == 0) sh[threadIdx.x >> 5] = v;
-  __syncthreads();
-  if (threadIdx.x < 32) {
-    uint64_t s = sh[threadIdx.x];
-    for (int o = 16; o; o >>= 1) s += __shfl_down_sync(0xffffffffu, s, o);
-    if (threadIdx.x == 0) sums[blockIdx.x] = s;
-  }
-}
-__global__ void k_scan_sums_inplace(uint64_t* sums, uint64_t nb) {
-  // single block; nb block sums -> exclusive prefix, chunked by blockDim
-  __shared__ uint64_t carry;
-  __shared__ uint64_t sh[1024];
-  if (threadIdx.x == 0) carry = 0;
-  __syncthreads();
-  for (uint64_t base = 0; base < nb; base += blockDim.x) {
-    uint64_t i = base + threadIdx.x;
-    uint64_t v = i < nb ? sums[i] : 0;
-    sh[threadIdx.x] = v;
-    __syncthreads();
-    for (int o = 1; o < blockDim.x; o <<= 1) {
-      uint64_t t = threadIdx.x >= o ? sh[threadIdx.x - o] : 0;
-      __syncthreads();
-      sh[threadIdx.x] += t;
-      __syncthreads();
-    }
-    uint64_t incl = sh[threadIdx.x];
-    if (i < nb) sums[i] = carry + incl - v;
-    __syncthreads();
-    if (threadIdx.x == blockDim.x - 1) carry += incl;
-    __syncthreads();
-  }
-}
-__global__ void k_scan_finish(const uint32_t* __restrict__ in, uint64_t n, const uint64_t* __restrict__ sums, uint64_t* __restrict__ out) {
-  __shared__ uint64_t sh[kScanBlock];
-  uint64_t i = blockIdx.x * (uint64_t)kScanBlock + threadIdx.x;
-  uint64_t v = i < n ? in[i] : 0;
-  sh[threadIdx.x] = v;
-  __syncthreads();
-  for (int o = 1; o < kScanBlock; o <<= 1) {
-    uint64_t t = threadIdx.x >= o ? sh[threadIdx.x - o] : 0;
-    __syncthreads();
-    sh[threadIdx.x] += t;
-    __syncthreads();
-  }
-  uint64_t excl = sums[blockIdx.x] + sh[threadIdx.x] - v;
-  if (i < n) out[i] = excl;
-  if (i == n - 1) out[n] = excl + v;
-}
-
-// out has n+1 entries.  tmp must hold ceil(n/1024) u64.
-int exclusive_scan_u32_u64(const uint32_t* in, uint64_t n, uint64_t* out, DevBuf& tmp, cudaStream_t s) {
-  if (n == 0) { FEI_CUDA(cudaMemsetAsync(out, 0, sizeof(uint64_t), s)); return FEI_OK; }
-  uint64_t nb = (n + kScanBlock - 1) / kScanBlock;
-  FEI_TRY(tmp.ensure(nb * sizeof(uint64_t)));
-  k_scan_block_sums<<<(unsigned)nb, kScanBlock, 0, s>>>(in, n, tmp.as<uint64_t>());
-  k_scan_sums_inplace<<<1, 1024, 0, s>>>(tmp.as<uint64_t>(), nb);
-  k_scan_finish<<<(unsigned)nb, kScanBlock, 0, s>>>(in, n, tmp.as<uint64_t>(), out);
-  FEI_CUDA(cudaGetLastError());
-  return FEI_OK;
-}
-
 static int chain_prepare(fei_chain* ch) {
   // msgs/msg_off/hash/hash_off/prev/prev_off are on the device: build padded blocks + link flags
   Context& c = ctx();
@@ -322,9 +253,8 @@ static int chain_prepare(fei_chain* ch) {
   FEI_TRY(ch->blk_off.ensure((n + 1) * sizeof(uint64_t)));
   unsigned g = (unsigned)((n + 255) / 256);
   k_count_blocks<<<g, 256, 0, c.stream>>>(ch->msg_off.as<uint64_t>(), n, ch->nblk.as<uint32_t>());
-  FEI_TRY(exclusive_scan_u32_u64(ch->nblk.as<uint32_t>(), n, ch->blk_off.as<uint64_t>(), ch->scan_tmp, c.stream));
   uint64_t total = 0;
-  FEI_CUDA(cudaMemcpyAsync(&total, ch->blk_off.as<uint64_t>() + n, sizeof(uint64_t), cudaMemcpyDeviceToHost, c.stream));
+  FEI_TRY(queue_offsets(ch->nblk.as<uint32_t>(), n, ch->blk_off.as<uint64_t>(), &total, false, ch->scan_tmp, c.stream));
   FEI_CUDA(cudaStreamSynchronize(c.stream));
   ch->total_blocks = total;
   FEI_TRY(ch->padded.ensure(total * 64));
@@ -496,14 +426,14 @@ struct DevCols { fei_json_col c[FEI_CHAIN_NCOLS]; };
 __global__ void __launch_bounds__(128) k_json_size(DevCols cols, uint64_t n, uint32_t* __restrict__ len, int* __restrict__ err) {
   const uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
   if (i >= n) return;
-  feijson::CountSink s;
+  CountSink s;
   if (feijson::put_block(s, cols.c, i) != 0) atomicExch(err, 1);
   len[i] = s.n;
 }
 __global__ void __launch_bounds__(128) k_json_write(DevCols cols, uint64_t n, const uint64_t* __restrict__ off, uint8_t* __restrict__ out) {
   const uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
   if (i >= n) return;
-  feijson::WriteSink s{out + off[i]};
+  WriteSink s{out + off[i]};
   feijson::put_block(s, cols.c, i);
 }
 }  // namespace fei
@@ -543,9 +473,8 @@ extern "C" int fei_chain_load_cols(fei_chain* ch, const fei_json_col* cols, cons
   FEI_TRY(ch->msg_off.ensure((n + 1) * 8));
   const unsigned g = (unsigned)((n + 127) / 128);
   k_json_size<<<g, 128, 0, s>>>(dc, n, ch->json_len.as<uint32_t>(), ch->json_err.as<int>());
-  FEI_TRY(exclusive_scan_u32_u64(ch->json_len.as<uint32_t>(), n, ch->msg_off.as<uint64_t>(), ch->scan_tmp, s));
   uint64_t total = 0; int err = 0;
-  FEI_CUDA(cudaMemcpyAsync(&total, ch->msg_off.as<uint64_t>() + n, 8, cudaMemcpyDeviceToHost, s));
+  FEI_TRY(queue_offsets(ch->json_len.as<uint32_t>(), n, ch->msg_off.as<uint64_t>(), &total, false, ch->scan_tmp, s));
   FEI_CUDA(cudaMemcpyAsync(&err, ch->json_err.p, 4, cudaMemcpyDeviceToHost, s));
   FEI_CUDA(cudaStreamSynchronize(s));                               // (also: the rebased offset vectors may go now)
   if (err) { set_error("unsupported JSON tag in chain columns"); return FEI_E_BADARG; }

@@ -27,7 +27,7 @@ static size_t block_bound(const fei_json_col* cols, uint64_t i) {
 // One block's text at dst; returns its end, or nullptr on an unsupported tag.  flatten inlines the whole writer so the sink's
 // pointer can live in a register; otherwise every byte store, which may alias the pointer, forces a store and reload of it.
 __attribute__((flatten)) static uint8_t* write_block(uint8_t* dst, const fei_json_col* cols, uint64_t i) {
-  feijson::WriteSink o{dst};
+  WriteSink o{dst};
   return feijson::put_block(o, cols, i) == 0 ? o.p : nullptr;
 }
 

@@ -57,6 +57,11 @@ struct DevBuf {
 // bytes behind them.
 int upload(DevBuf& b, const void* src, size_t bytes, size_t zero_slack, cudaStream_t s);
 
+// The offsets step of the calls that size items, place them and then write them: queues on s the exclusive scan of len[0..n) into
+// off[0..n] (off[n] = the total) and the copy to the host of all of off[0..n] (whole) or of off[n] alone, into `host`.  Nothing
+// waits: the caller queues its other read-backs and synchronises once.
+int queue_offsets(const uint32_t* len, uint64_t n, uint64_t* off, uint64_t* host, bool whole, DevBuf& tmp, cudaStream_t s);
+
 // process-wide state
 struct Context {
   int device = -1;

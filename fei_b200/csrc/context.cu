@@ -50,6 +50,81 @@ int upload(DevBuf& b, const void* src, size_t bytes, size_t zero_slack, cudaStre
   return FEI_OK;
 }
 
+// Simple three-phase exclusive scan of u32 -> u64 (n up to 2^40): per-block sums,
+// serial scan of the block sums by one thread block, then per-block rescan.
+constexpr int kScanBlock = 1024;
+__global__ void k_scan_block_sums(const uint32_t* __restrict__ in, uint64_t n, uint64_t* __restrict__ sums) {
+  __shared__ uint64_t sh[32];
+  uint64_t i = blockIdx.x * (uint64_t)kScanBlock + threadIdx.x;
+  uint64_t v = i < n ? in[i] : 0;
+  for (int o = 16; o; o >>= 1) v += __shfl_down_sync(0xffffffffu, v, o);
+  if ((threadIdx.x & 31) == 0) sh[threadIdx.x >> 5] = v;
+  __syncthreads();
+  if (threadIdx.x < 32) {
+    uint64_t s = sh[threadIdx.x];
+    for (int o = 16; o; o >>= 1) s += __shfl_down_sync(0xffffffffu, s, o);
+    if (threadIdx.x == 0) sums[blockIdx.x] = s;
+  }
+}
+__global__ void k_scan_sums_inplace(uint64_t* sums, uint64_t nb) {
+  // single block; nb block sums -> exclusive prefix, chunked by blockDim
+  __shared__ uint64_t carry;
+  __shared__ uint64_t sh[1024];
+  if (threadIdx.x == 0) carry = 0;
+  __syncthreads();
+  for (uint64_t base = 0; base < nb; base += blockDim.x) {
+    uint64_t i = base + threadIdx.x;
+    uint64_t v = i < nb ? sums[i] : 0;
+    sh[threadIdx.x] = v;
+    __syncthreads();
+    for (int o = 1; o < blockDim.x; o <<= 1) {
+      uint64_t t = threadIdx.x >= o ? sh[threadIdx.x - o] : 0;
+      __syncthreads();
+      sh[threadIdx.x] += t;
+      __syncthreads();
+    }
+    uint64_t incl = sh[threadIdx.x];
+    if (i < nb) sums[i] = carry + incl - v;
+    __syncthreads();
+    if (threadIdx.x == blockDim.x - 1) carry += incl;
+    __syncthreads();
+  }
+}
+__global__ void k_scan_finish(const uint32_t* __restrict__ in, uint64_t n, const uint64_t* __restrict__ sums, uint64_t* __restrict__ out) {
+  __shared__ uint64_t sh[kScanBlock];
+  uint64_t i = blockIdx.x * (uint64_t)kScanBlock + threadIdx.x;
+  uint64_t v = i < n ? in[i] : 0;
+  sh[threadIdx.x] = v;
+  __syncthreads();
+  for (int o = 1; o < kScanBlock; o <<= 1) {
+    uint64_t t = threadIdx.x >= o ? sh[threadIdx.x - o] : 0;
+    __syncthreads();
+    sh[threadIdx.x] += t;
+    __syncthreads();
+  }
+  uint64_t excl = sums[blockIdx.x] + sh[threadIdx.x] - v;
+  if (i < n) out[i] = excl;
+  if (i == n - 1) out[n] = excl + v;
+}
+
+// out has n+1 entries.  tmp grows to ceil(n/1024) u64.
+static int exclusive_scan_u32_u64(const uint32_t* in, uint64_t n, uint64_t* out, DevBuf& tmp, cudaStream_t s) {
+  if (n == 0) { FEI_CUDA(cudaMemsetAsync(out, 0, sizeof(uint64_t), s)); return FEI_OK; }
+  uint64_t nb = (n + kScanBlock - 1) / kScanBlock;
+  FEI_TRY(tmp.ensure(nb * sizeof(uint64_t)));
+  k_scan_block_sums<<<(unsigned)nb, kScanBlock, 0, s>>>(in, n, tmp.as<uint64_t>());
+  k_scan_sums_inplace<<<1, 1024, 0, s>>>(tmp.as<uint64_t>(), nb);
+  k_scan_finish<<<(unsigned)nb, kScanBlock, 0, s>>>(in, n, tmp.as<uint64_t>(), out);
+  FEI_CUDA(cudaGetLastError());
+  return FEI_OK;
+}
+
+int queue_offsets(const uint32_t* len, uint64_t n, uint64_t* off, uint64_t* host, bool whole, DevBuf& tmp, cudaStream_t s) {
+  FEI_TRY(exclusive_scan_u32_u64(len, n, off, tmp, s));
+  FEI_CUDA(cudaMemcpyAsync(host, whole ? off : off + n, (whole ? n + 1 : 1) * sizeof(uint64_t), cudaMemcpyDeviceToHost, s));
+  return FEI_OK;
+}
+
 /* The CUDA "current device" is per host thread: a worker thread of the caller (a thread pool loading batches, Flask's request
  * threads) starts on device 0 whatever fei_init bound.  Every path that touches the device goes through ctx() or DevBuf::alloc, so
  * this is where the calling thread is put on the bound device. */

@@ -132,47 +132,26 @@ __global__ void k_untile_idx(const uint8_t* __restrict__ tiles, const uint64_t* 
   }
 }
 
-// Offsets [m + 1] of the fetched records' headers and bodies, computed on the device: into d_hoff / d_boff for the copy
-// kernels and into hdr_off / body_off on the host.  Synchronises s.
-static int fetch_offsets(fei_corpus* c, const uint64_t* d_idx, uint64_t first, uint64_t m, DevBuf& d_hoff, DevBuf& d_boff,
-                         uint64_t* hdr_off, uint64_t* body_off, cudaStream_t s) {
+int fetch_offsets(fei_corpus* c, const uint64_t* d_idx, uint64_t first, uint64_t m, DevBuf* d_hoff, DevBuf& d_boff,
+                  uint64_t* hdr_off, uint64_t* body_off, bool whole, cudaStream_t s) {
   DevBuf d_hlen, d_blen;
-  FEI_TRY(d_hlen.alloc(m * 4)); FEI_TRY(d_blen.alloc(m * 4)); FEI_TRY(d_hoff.alloc((m + 1) * 8)); FEI_TRY(d_boff.alloc((m + 1) * 8));
+  FEI_TRY(d_hlen.alloc(m * 4)); FEI_TRY(d_blen.alloc(m * 4)); FEI_TRY(d_boff.alloc((m + 1) * 8));
   k_rec_lens<<<(unsigned)((m + 127) / 128), 128, 0, s>>>(d_idx, first, m, c->hdr_off.as<uint64_t>(), c->rec_pos.as<uint32_t>(), c->grp_len.as<uint32_t>(),
                                                          d_hlen.as<uint32_t>(), d_blen.as<uint32_t>());
-  FEI_TRY(exclusive_scan_u32_u64(d_hlen.as<uint32_t>(), m, d_hoff.as<uint64_t>(), c->scan_tmp, s));
-  FEI_TRY(exclusive_scan_u32_u64(d_blen.as<uint32_t>(), m, d_boff.as<uint64_t>(), c->scan_tmp, s));
-  FEI_CUDA(cudaMemcpyAsync(hdr_off, d_hoff.p, (m + 1) * 8, cudaMemcpyDeviceToHost, s));
-  FEI_CUDA(cudaMemcpyAsync(body_off, d_boff.p, (m + 1) * 8, cudaMemcpyDeviceToHost, s));
+  if (d_hoff) {
+    FEI_TRY(d_hoff->alloc((m + 1) * 8));
+    FEI_TRY(queue_offsets(d_hlen.as<uint32_t>(), m, d_hoff->as<uint64_t>(), hdr_off, whole, c->scan_tmp, s));
+  }
+  FEI_TRY(queue_offsets(d_blen.as<uint32_t>(), m, d_boff.as<uint64_t>(), body_off, whole, c->scan_tmp, s));
   FEI_CUDA(cudaStreamSynchronize(s));
   return FEI_OK;
 }
 
-// The bodies of the fetched records, un-tiled on the device into body[0, bytes).  Synchronises s.
-static int fetch_bodies(fei_corpus* c, const uint64_t* d_idx, uint64_t first, uint64_t m, const DevBuf& d_boff, uint8_t* body, uint64_t bytes,
-                        cudaStream_t s) {
-  DevBuf d_b;
-  FEI_TRY(d_b.alloc(bytes + 16));
+int untile_bodies(fei_corpus* c, const uint64_t* d_idx, uint64_t first, uint64_t m, const DevBuf& d_boff, uint64_t bytes, DevBuf& d_body,
+                  cudaStream_t s) {
+  FEI_TRY(d_body.alloc(bytes + 16));
   k_untile_idx<<<(unsigned)((m + 127) / 128), 128, 0, s>>>(c->tiles.as<uint8_t>(), c->grp_base.as<uint64_t>(), c->grp_len.as<uint32_t>(), c->rec_pos.as<uint32_t>(),
-                                                           d_idx, first, m, d_boff.as<uint64_t>(), d_b.as<uint8_t>());
-  FEI_CUDA(cudaGetLastError());
-  FEI_CUDA(cudaMemcpyAsync(body, d_b.p, bytes, cudaMemcpyDeviceToHost, s));
-  FEI_CUDA(cudaStreamSynchronize(s));
-  return FEI_OK;
-}
-
-int untile_bodies(fei_corpus* c, const uint64_t* d_idx, uint64_t m, DevBuf& d_boff, DevBuf& d_body, cudaStream_t s) {
-  DevBuf d_hlen, d_blen;
-  FEI_TRY(d_hlen.alloc(m * 4 + 4)); FEI_TRY(d_blen.alloc(m * 4 + 4)); FEI_TRY(d_boff.alloc((m + 1) * 8));
-  if (m) k_rec_lens<<<(unsigned)((m + 127) / 128), 128, 0, s>>>(d_idx, 0, m, c->hdr_off.as<uint64_t>(), c->rec_pos.as<uint32_t>(), c->grp_len.as<uint32_t>(),
-                                                                d_hlen.as<uint32_t>(), d_blen.as<uint32_t>());
-  FEI_TRY(exclusive_scan_u32_u64(d_blen.as<uint32_t>(), m, d_boff.as<uint64_t>(), c->scan_tmp, s));
-  uint64_t total = 0;
-  FEI_CUDA(cudaMemcpyAsync(&total, d_boff.as<uint64_t>() + m, 8, cudaMemcpyDeviceToHost, s));
-  FEI_CUDA(cudaStreamSynchronize(s));
-  FEI_TRY(d_body.alloc(total + 16));
-  if (m) k_untile_idx<<<(unsigned)((m + 127) / 128), 128, 0, s>>>(c->tiles.as<uint8_t>(), c->grp_base.as<uint64_t>(), c->grp_len.as<uint32_t>(), c->rec_pos.as<uint32_t>(),
-                                                                  d_idx, 0, m, d_boff.as<uint64_t>(), d_body.as<uint8_t>());
+                                                           d_idx, first, m, d_boff.as<uint64_t>(), d_body.as<uint8_t>());
   FEI_CUDA(cudaGetLastError());
   return FEI_OK;
 }
@@ -203,9 +182,8 @@ static int build_tiles(fei_corpus* c, const uint8_t* d_body, const uint64_t* d_b
   k_units<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(d_body_off, n, len.as<uint32_t>());
   k_window_sort<<<(unsigned)n_windows, kSortThreads, 0, s>>>(len.as<uint32_t>(), n, c->grp_rec.as<uint32_t>(), c->grp_len.as<uint32_t>(),
                                                        gunits.as<uint32_t>(), c->rec_pos.as<uint32_t>());
-  FEI_TRY(exclusive_scan_u32_u64(gunits.as<uint32_t>(), n_groups, c->grp_base.as<uint64_t>(), c->scan_tmp, s));
   uint64_t total_units = 0;
-  FEI_CUDA(cudaMemcpyAsync(&total_units, c->grp_base.as<uint64_t>() + n_groups, 8, cudaMemcpyDeviceToHost, s));
+  FEI_TRY(queue_offsets(gunits.as<uint32_t>(), n_groups, c->grp_base.as<uint64_t>(), &total_units, false, c->scan_tmp, s));
   FEI_CUDA(cudaStreamSynchronize(s));
   c->tile_bytes = total_units * 16;
   FEI_TRY(c->tiles.ensure(c->tile_bytes + 64));
@@ -221,8 +199,8 @@ static int build_tiles(fei_corpus* c, const uint8_t* d_body, const uint64_t* d_b
 __global__ void k_synth_len(uint64_t seed, uint64_t first, uint64_t n, uint32_t* __restrict__ hlen, uint32_t* __restrict__ blen) {
   uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
   if (i >= n) return;
-  feisynth::CountSink ch; feisynth::gen_header(ch, seed, first + i);
-  feisynth::CountSink cb; feisynth::gen_body(cb, seed, first + i);
+  CountSink ch; feisynth::gen_header(ch, seed, first + i);
+  CountSink cb; feisynth::gen_body(cb, seed, first + i);
   hlen[i] = ch.n; blen[i] = cb.n;
 }
 
@@ -231,8 +209,8 @@ __global__ void k_synth_write(uint64_t seed, uint64_t first, uint64_t n, const u
                               int64_t* __restrict__ ts, int64_t* __restrict__ wall, uint64_t* __restrict__ flags8, uint32_t* __restrict__ fsb) {
   uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
   if (i >= n) return;
-  { feisynth::WriteSink w(hdr + hoff[i]); feisynth::gen_header(w, seed, first + i); }
-  { feisynth::WriteSink w(body + boff[i]); feisynth::gen_body(w, seed, first + i); }
+  { WriteSink w{hdr + hoff[i]}; feisynth::gen_header(w, seed, first + i); }
+  { WriteSink w{body + boff[i]}; feisynth::gen_body(w, seed, first + i); }
   feisynth::RecMeta m = feisynth::gen_meta(seed, first + i);
   ts[i] = m.ts; wall[i] = m.ts;                              // synthetic corpora live in UTC
   uint64_t f = 0;
@@ -245,6 +223,17 @@ int check_load(uint64_t n, const fei_corpus_host* h) {
   FEI_TRY(require_ready());
   if (n >= 0xFFFFFFFFull) { set_error("at most 2^32-2 records per shard"); return FEI_E_BADARG; }
   if (h && n && (!h->ts || !h->wall || !h->flags8 || !h->fsb)) { set_error("missing meta array"); return FEI_E_BADARG; }
+  return FEI_OK;
+}
+
+int require_loaded(const fei_corpus* c) {
+  FEI_TRY(require_ready());
+  if (!c || !c->loaded) { set_error("corpus not loaded"); return FEI_E_STATE; }
+  return FEI_OK;
+}
+
+int check_record_indices(const fei_corpus* c, const uint64_t* idx, uint64_t m) {
+  for (uint64_t i = 0; i < m; ++i) if (idx[i] >= c->n) { set_error("record index %llu out of range", (unsigned long long)idx[i]); return FEI_E_BADARG; }
   return FEI_OK;
 }
 
@@ -341,11 +330,9 @@ extern "C" int fei_corpus_synth(fei_corpus* c, uint64_t seed, uint64_t first, ui
   FEI_TRY(c->ts.alloc(n1 * 8)); FEI_TRY(c->wall.alloc(n1 * 8)); FEI_TRY(c->flags8.alloc(n1 * 8)); FEI_TRY(c->fsb.alloc(n1 * 4));
   unsigned g = (unsigned)((n + 127) / 128);
   if (n) k_synth_len<<<g, 128, 0, s>>>(seed, first, n, hlen.as<uint32_t>(), blen.as<uint32_t>());
-  FEI_TRY(exclusive_scan_u32_u64(hlen.as<uint32_t>(), n, c->hdr_off.as<uint64_t>(), c->scan_tmp, s));
-  FEI_TRY(exclusive_scan_u32_u64(blen.as<uint32_t>(), n, body_off.as<uint64_t>(), c->scan_tmp, s));
   uint64_t hb = 0, bb = 0;
-  FEI_CUDA(cudaMemcpyAsync(&hb, c->hdr_off.as<uint64_t>() + n, 8, cudaMemcpyDeviceToHost, s));
-  FEI_CUDA(cudaMemcpyAsync(&bb, body_off.as<uint64_t>() + n, 8, cudaMemcpyDeviceToHost, s));
+  FEI_TRY(queue_offsets(hlen.as<uint32_t>(), n, c->hdr_off.as<uint64_t>(), &hb, false, c->scan_tmp, s));
+  FEI_TRY(queue_offsets(blen.as<uint32_t>(), n, body_off.as<uint64_t>(), &bb, false, c->scan_tmp, s));
   FEI_CUDA(cudaStreamSynchronize(s));
   hlen.release(); blen.release();
   c->hdr_bytes = hb; c->body_bytes = bb;
@@ -375,18 +362,17 @@ extern "C" int fei_corpus_fetch(fei_corpus* c, uint64_t first, uint64_t n,
                                 int64_t* ts, int64_t* wall, uint64_t* flags8, uint32_t* fsb) {
   if (!c) { set_error("null corpus"); return FEI_E_BADARG; }
   std::lock_guard<std::mutex> lock(c->mu);
-  FEI_TRY(require_ready());
-  if (!c->loaded) { set_error("corpus not loaded"); return FEI_E_STATE; }
+  FEI_TRY(require_loaded(c));
   if (first + n > c->n) { set_error("range out of bounds"); return FEI_E_BADARG; }
   if (n == 0) return FEI_OK;
   cudaStream_t s = ctx().stream;
   uint64_t h0 = 0;
   std::vector<uint64_t> ho, bo;
-  DevBuf d_hoff, d_boff;
+  DevBuf d_hoff, d_boff, d_body;
   if (hdr || hdr_off || body || body_off) {          // not for the meta columns alone
     ho.resize(n + 1); bo.resize(n + 1);
     FEI_CUDA(cudaMemcpyAsync(&h0, c->hdr_off.as<uint64_t>() + first, 8, cudaMemcpyDeviceToHost, s));
-    FEI_TRY(fetch_offsets(c, nullptr, first, n, d_hoff, d_boff, ho.data(), bo.data(), s));
+    FEI_TRY(fetch_offsets(c, nullptr, first, n, &d_hoff, d_boff, ho.data(), bo.data(), true, s));
   }
   if (hdr_off) memcpy(hdr_off, ho.data(), (n + 1) * 8);
   if (hdr) {
@@ -400,7 +386,8 @@ extern "C" int fei_corpus_fetch(fei_corpus* c, uint64_t first, uint64_t n,
   if (body_off) memcpy(body_off, bo.data(), (n + 1) * 8);
   if (body) {
     if (bo[n] > body_cap) { set_error("body buffer too small: need %llu", (unsigned long long)bo[n]); return FEI_E_CAPACITY; }
-    FEI_TRY(fetch_bodies(c, nullptr, first, n, d_boff, body, bo[n], s));
+    FEI_TRY(untile_bodies(c, nullptr, first, n, d_boff, bo[n], d_body, s));
+    FEI_CUDA(cudaMemcpyAsync(body, d_body.p, bo[n], cudaMemcpyDeviceToHost, s));
   }
   FEI_CUDA(cudaStreamSynchronize(s));
   return FEI_OK;
@@ -413,23 +400,25 @@ extern "C" int fei_corpus_fetch_records(fei_corpus* c, const uint64_t* idx, uint
                                         uint8_t* body, uint64_t body_cap, uint64_t* body_off) {
   if (!c || (m && !idx) || !hdr_off || !body_off) { set_error("null argument"); return FEI_E_BADARG; }
   std::lock_guard<std::mutex> lock(c->mu);
-  FEI_TRY(require_ready());
-  if (!c->loaded) { set_error("corpus not loaded"); return FEI_E_STATE; }
+  FEI_TRY(require_loaded(c));
   hdr_off[0] = 0; body_off[0] = 0;
   if (m == 0) return FEI_OK;
-  for (uint64_t i = 0; i < m; ++i) if (idx[i] >= c->n) { set_error("record index %llu out of range", (unsigned long long)idx[i]); return FEI_E_BADARG; }
+  FEI_TRY(check_record_indices(c, idx, m));
   cudaStream_t s = ctx().stream;
-  DevBuf d_idx, d_hoff, d_boff, d_h;
+  DevBuf d_idx, d_hoff, d_boff, d_h, d_body;
   FEI_TRY(d_idx.alloc(m * 8));
   FEI_CUDA(cudaMemcpyAsync(d_idx.p, idx, m * 8, cudaMemcpyHostToDevice, s));
-  FEI_TRY(fetch_offsets(c, d_idx.as<uint64_t>(), 0, m, d_hoff, d_boff, hdr_off, body_off, s));
+  FEI_TRY(fetch_offsets(c, d_idx.as<uint64_t>(), 0, m, &d_hoff, d_boff, hdr_off, body_off, true, s));
   if ((hdr && hdr_off[m] > hdr_cap) || (body && body_off[m] > body_cap)) { set_error("fetch buffers too small: need %llu header and %llu body bytes", (unsigned long long)hdr_off[m], (unsigned long long)body_off[m]); return FEI_E_CAPACITY; }
   if (hdr && hdr_off[m]) {
     FEI_TRY(d_h.alloc(hdr_off[m] + 16));
     k_copy_hdr<<<(unsigned)((m * 32 + 255) / 256), 256, 0, s>>>(d_idx.as<uint64_t>(), m, c->hdr.as<uint8_t>(), c->hdr_off.as<uint64_t>(), d_hoff.as<uint64_t>(), d_h.as<uint8_t>());
     FEI_CUDA(cudaMemcpyAsync(hdr, d_h.p, hdr_off[m], cudaMemcpyDeviceToHost, s));
   }
-  if (body && body_off[m]) FEI_TRY(fetch_bodies(c, d_idx.as<uint64_t>(), 0, m, d_boff, body, body_off[m], s));
+  if (body && body_off[m]) {
+    FEI_TRY(untile_bodies(c, d_idx.as<uint64_t>(), 0, m, d_boff, body_off[m], d_body, s));
+    FEI_CUDA(cudaMemcpyAsync(body, d_body.p, body_off[m], cudaMemcpyDeviceToHost, s));
+  }
   FEI_CUDA(cudaStreamSynchronize(s));
   FEI_CUDA(cudaGetLastError());
   return FEI_OK;

@@ -104,6 +104,10 @@ cudaStream_t corpus_load_stream(fei_corpus* c);   // created on first use; falls
 // Checks every load makes before it touches the handle (caller holds c->mu): the device is bound, n fits the tiles' 32-bit
 // record indices and, when h is given, the meta arrays are there.
 int check_load(uint64_t n, const fei_corpus_host* h);
+// Checks of the calls that read a corpus (caller holds c->mu): the device is bound and c holds a loaded corpus; every idx[0..m) is
+// one of its records.
+int require_loaded(const fei_corpus* c);
+int check_record_indices(const fei_corpus* c, const uint64_t* idx, uint64_t m);
 // ts / wall / flags8 / fsb and the optional names of h, queued on s
 int upload_meta(fei_corpus* c, const fei_corpus_host* h, cudaStream_t s);
 // The end of every load: tiles from the canonical body on the device (kBlobSlack zeroed bytes behind it), then the header
@@ -111,10 +115,13 @@ int upload_meta(fei_corpus* c, const fei_corpus_host* h, cudaStream_t s);
 int pack_canonical(fei_corpus* c, DevBuf& body, DevBuf& body_off, cudaStream_t s, bool drop_text, cudaEvent_t packed);
 // builds the header directory from hdr / hdr_off already on the device (hdir.cu)
 int build_header_dir(fei_corpus* c, cudaStream_t s);
-int exclusive_scan_u32_u64(const uint32_t* in, uint64_t n, uint64_t* out, DevBuf& tmp, cudaStream_t s);
-// The bodies of records d_idx[0..m) (device array) un-tiled on the device: d_boff gets their m + 1 offsets, d_body the bytes
-// (k_rec_lens, a scan and k_untile_idx, queued on s after one wait for the total).
-int untile_bodies(fei_corpus* c, const uint64_t* d_idx, uint64_t m, DevBuf& d_boff, DevBuf& d_body, cudaStream_t s);
+// Fetched records are d_idx[0..m) (device array), or first + i when d_idx is null.  fetch_offsets places their bodies, and their
+// headers when d_hoff is given, into d_boff / d_hoff [m + 1] and copies to body_off / hdr_off on the host every offset (whole) or
+// the total alone; it synchronises s.  untile_bodies then queues the bodies' `bytes` (d_boff[m]) into d_body on s.
+int fetch_offsets(fei_corpus* c, const uint64_t* d_idx, uint64_t first, uint64_t m, DevBuf* d_hoff, DevBuf& d_boff,
+                  uint64_t* hdr_off, uint64_t* body_off, bool whole, cudaStream_t s);
+int untile_bodies(fei_corpus* c, const uint64_t* d_idx, uint64_t first, uint64_t m, const DevBuf& d_boff, uint64_t bytes, DevBuf& d_body,
+                  cudaStream_t s);
 // Multi-GPU exchange of a scan (comm.cu).
 struct ScanHook {
   // if set, the scan kernel itself stores every finished window's hit masks into these peer buffers (device array of push_n

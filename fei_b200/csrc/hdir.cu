@@ -162,9 +162,8 @@ int build_header_dir(fei_corpus* c, cudaStream_t s) {
     FEI_CUDA(cudaMemsetAsync(kd.rep, 0xFF, kKeySlots * sizeof(unsigned long long), s));
     FEI_CUDA(cudaMemsetAsync(kd.len, 0, (2 * kKeySlots + 2) * sizeof(uint32_t), s));
     k_hdir<0><<<blocks, 256, 0, s>>>(c->hdr.as<uint8_t>(), c->hdr_off.as<uint64_t>(), n, cnt.as<uint32_t>(), nullptr, nullptr, kd, force_text);
-    FEI_TRY(exclusive_scan_u32_u64(cnt.as<uint32_t>(), n, c->hdir_off.as<uint64_t>(), c->scan_tmp, s));
     uint64_t total = 0;
-    FEI_CUDA(cudaMemcpyAsync(&total, c->hdir_off.as<uint64_t>() + n, 8, cudaMemcpyDeviceToHost, s));
+    FEI_TRY(queue_offsets(cnt.as<uint32_t>(), n, c->hdir_off.as<uint64_t>(), &total, false, c->scan_tmp, s));
     FEI_CUDA(cudaStreamSynchronize(s));
     c->hdir_entries = total;
     FEI_TRY(c->hdir.ensure((total + 1) * sizeof(uint2)));

@@ -303,13 +303,11 @@ static int load_raw_impl(fei_corpus* c, const fei_corpus_host* h, const uint8_t*
   FEI_TRY(c->hdr_off.ensure((n + 1) * 8));
   DevBuf& body_off = c->stage_body_off; DevBuf& body = c->stage_body;
   FEI_TRY(body_off.ensure((n + 1) * 8));
-  FEI_TRY(exclusive_scan_u32_u64(d_hlen.as<uint32_t>(), n, c->hdr_off.as<uint64_t>(), c->scan_tmp, s));
-  FEI_TRY(exclusive_scan_u32_u64(d_blen.as<uint32_t>(), n, body_off.as<uint64_t>(), c->scan_tmp, s));
   unsigned long long summary[2] = {0, 0};
   uint64_t hb = 0, bb = 0;
+  FEI_TRY(queue_offsets(d_hlen.as<uint32_t>(), n, c->hdr_off.as<uint64_t>(), &hb, false, c->scan_tmp, s));
+  FEI_TRY(queue_offsets(d_blen.as<uint32_t>(), n, body_off.as<uint64_t>(), &bb, false, c->scan_tmp, s));
   FEI_CUDA(cudaMemcpyAsync(summary, d_summary, 16, cudaMemcpyDeviceToHost, s));
-  FEI_CUDA(cudaMemcpyAsync(&hb, c->hdr_off.as<uint64_t>() + n, 8, cudaMemcpyDeviceToHost, s));
-  FEI_CUDA(cudaMemcpyAsync(&bb, body_off.as<uint64_t>() + n, 8, cudaMemcpyDeviceToHost, s));
   FEI_CUDA(cudaStreamSynchronize(s));
   if (summary[0]) {
     if (valid_out) {

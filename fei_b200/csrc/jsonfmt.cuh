@@ -7,16 +7,11 @@
 #include <stdint.h>
 #include <string.h>
 #include "../../include/feiscan.h"
-
-#if defined(__CUDACC__)
-#define FEI_JHD __host__ __device__ __forceinline__
-#define FEI_JHD_NI __host__ __device__ inline
-#else
-#define FEI_JHD inline
-#define FEI_JHD_NI inline
-#endif
+#include "sink.cuh"
 
 namespace feijson {
+using fei::put_bytes;
+using fei::put_lit;
 
 #define FEI_RYU_TABLE static const
 namespace tab_host {
@@ -31,14 +26,14 @@ namespace tab_dev {
 #undef FEI_RYU_TABLE
 #endif
 
-FEI_JHD const uint64_t* pow5_inv(int i) {
+FEI_HD const uint64_t* pow5_inv(int i) {
 #if defined(__CUDA_ARCH__)
   return tab_dev::kRyuPow5Inv[i];
 #else
   return tab_host::kRyuPow5Inv[i];
 #endif
 }
-FEI_JHD const uint64_t* pow5(int i) {
+FEI_HD const uint64_t* pow5(int i) {
 #if defined(__CUDA_ARCH__)
   return tab_dev::kRyuPow5[i];
 #else
@@ -46,15 +41,8 @@ FEI_JHD const uint64_t* pow5(int i) {
 #endif
 }
 
-// ---------------------------------------------------------------- sinks
-struct CountSink { uint32_t n = 0; FEI_JHD void put(uint8_t) { ++n; } };
-struct WriteSink { uint8_t* p; FEI_JHD void put(uint8_t c) { *p++ = c; } };
-
-template <class S> FEI_JHD void put_lit(S& o, const char* s) { while (*s) o.put((uint8_t)*s++); }
-template <class S> FEI_JHD void put_bytes(S& o, const uint8_t* s, uint64_t n) { for (uint64_t i = 0; i < n; ++i) o.put(s[i]); }
-
 // ---------------------------------------------------------------- Ryu: double -> shortest decimal (digits, exponent)
-FEI_JHD uint64_t umul128(uint64_t a, uint64_t b, uint64_t* hi) {
+FEI_HD uint64_t umul128(uint64_t a, uint64_t b, uint64_t* hi) {
 #if defined(__CUDA_ARCH__)
   *hi = __umul64hi(a, b);
   return a * b;
@@ -64,8 +52,8 @@ FEI_JHD uint64_t umul128(uint64_t a, uint64_t b, uint64_t* hi) {
   return (uint64_t)p;
 #endif
 }
-FEI_JHD uint64_t shiftright128(uint64_t lo, uint64_t hi, uint32_t dist) { return (hi << (64 - dist)) | (lo >> dist); }   // 0 < dist < 64
-FEI_JHD uint64_t mul_shift64(uint64_t m, const uint64_t* mul, int j) {
+FEI_HD uint64_t shiftright128(uint64_t lo, uint64_t hi, uint32_t dist) { return (hi << (64 - dist)) | (lo >> dist); }   // 0 < dist < 64
+FEI_HD uint64_t mul_shift64(uint64_t m, const uint64_t* mul, int j) {
   uint64_t high1, high0;
   const uint64_t low1 = umul128(m, mul[1], &high1);
   umul128(m, mul[0], &high0);
@@ -73,15 +61,15 @@ FEI_JHD uint64_t mul_shift64(uint64_t m, const uint64_t* mul, int j) {
   if (sum < high0) ++high1;
   return shiftright128(sum, high1, (uint32_t)(j - 64));
 }
-FEI_JHD uint32_t pow5_factor(uint64_t v) { uint32_t c = 0; while (v && v % 5 == 0) { v /= 5; ++c; } return c; }
-FEI_JHD bool multiple_of_pow5(uint64_t v, uint32_t p) { return pow5_factor(v) >= p; }
-FEI_JHD bool multiple_of_pow2(uint64_t v, uint32_t p) { return (v & ((1ull << p) - 1)) == 0; }
-FEI_JHD int pow5bits(int e) { return (int)(((uint32_t)e * 1217359u) >> 19) + 1; }
-FEI_JHD int log10_pow2(int e) { return (int)(((uint32_t)e * 78913u) >> 18); }
-FEI_JHD int log10_pow5(int e) { return (int)(((uint32_t)e * 732923u) >> 20); }
+FEI_HD uint32_t pow5_factor(uint64_t v) { uint32_t c = 0; while (v && v % 5 == 0) { v /= 5; ++c; } return c; }
+FEI_HD bool multiple_of_pow5(uint64_t v, uint32_t p) { return pow5_factor(v) >= p; }
+FEI_HD bool multiple_of_pow2(uint64_t v, uint32_t p) { return (v & ((1ull << p) - 1)) == 0; }
+FEI_HD int pow5bits(int e) { return (int)(((uint32_t)e * 1217359u) >> 19) + 1; }
+FEI_HD int log10_pow2(int e) { return (int)(((uint32_t)e * 78913u) >> 18); }
+FEI_HD int log10_pow5(int e) { return (int)(((uint32_t)e * 732923u) >> 20); }
 
 // value = mantissa * 10^exponent, mantissa without trailing zeros beyond what shortest round-trip leaves
-FEI_JHD_NI void ryu_d2d(uint64_t ieee_mantissa, uint32_t ieee_exponent, uint64_t* out_mantissa, int* out_exponent) {
+FEI_HD_NI void ryu_d2d(uint64_t ieee_mantissa, uint32_t ieee_exponent, uint64_t* out_mantissa, int* out_exponent) {
   const int kMant = 52, kBias = 1023;
   int e2; uint64_t m2;
   if (ieee_exponent == 0) { e2 = 1 - kBias - kMant - 2; m2 = ieee_mantissa; }
@@ -153,7 +141,7 @@ FEI_JHD_NI void ryu_d2d(uint64_t ieee_mantissa, uint32_t ieee_exponent, uint64_t
 
 // float.__repr__: exponent form iff decpt <= -4 or decpt > 16; ".0" appended to integers; exponent of at least two digits.
 // json.dumps spells the non-finite values NaN / Infinity / -Infinity (allow_nan=True).
-template <class S> FEI_JHD_NI void put_float(S& o, uint64_t bits) {
+template <class S> FEI_HD_NI void put_float(S& o, uint64_t bits) {
   const bool neg = (bits >> 63) != 0;
   const uint64_t mant = bits & ((1ull << 52) - 1);
   const uint32_t expo = (uint32_t)((bits >> 52) & 0x7FF);
@@ -192,7 +180,7 @@ template <class S> FEI_JHD_NI void put_float(S& o, uint64_t bits) {
   }
 }
 
-template <class S> FEI_JHD void put_int(S& o, int64_t v) {
+template <class S> FEI_HD void put_int(S& o, int64_t v) {
   uint64_t u = v < 0 ? 0ull - (uint64_t)v : (uint64_t)v;
   if (v < 0) o.put('-');
   char tmp[20]; int k = 0;
@@ -200,14 +188,14 @@ template <class S> FEI_JHD void put_int(S& o, int64_t v) {
   while (k) o.put((uint8_t)tmp[--k]);
 }
 
-template <class S> FEI_JHD void put_u4(S& o, uint32_t cp) {      // \uXXXX, lowercase hex like json.encoder
+template <class S> FEI_HD void put_u4(S& o, uint32_t cp) {      // \uXXXX, lowercase hex like json.encoder
   const char* hx = "0123456789abcdef";
   o.put('\\'); o.put('u'); o.put((uint8_t)hx[(cp >> 12) & 15]); o.put((uint8_t)hx[(cp >> 8) & 15]); o.put((uint8_t)hx[(cp >> 4) & 15]); o.put((uint8_t)hx[cp & 15]);
 }
 
 // one ASCII character as py_encode_basestring_ascii writes it (put_json_string keeps its own copy of this switch: routing it
 // through here changes the SASS of the chain kernels that instantiate it)
-template <class S> FEI_JHD void put_json_ascii(S& o, uint32_t c) {
+template <class S> FEI_HD void put_json_ascii(S& o, uint32_t c) {
   switch (c) {
     case '"': o.put('\\'); o.put('"'); break;
     case '\\': o.put('\\'); o.put('\\'); break;
@@ -222,7 +210,7 @@ template <class S> FEI_JHD void put_json_ascii(S& o, uint32_t c) {
 
 // py_encode_basestring_ascii: everything outside ' '..'~' plus '"' and '\\' is escaped.  Input is UTF-8 (lone surrogates
 // arrive as 3-byte "surrogatepass" sequences).
-template <class S> FEI_JHD_NI void put_json_string(S& o, const uint8_t* s, uint64_t n) {
+template <class S> FEI_HD_NI void put_json_string(S& o, const uint8_t* s, uint64_t n) {
   o.put('"');
   uint64_t i = 0;
   while (i < n) {
@@ -255,7 +243,7 @@ template <class S> FEI_JHD_NI void put_json_string(S& o, const uint8_t* s, uint6
 
 // Length of the well-formed UTF-8 sequence at s[0..n) (Python's strict decoder: no overlongs, surrogates or code points past
 // U+10FFFF), or 0 when s[0] does not start one.
-FEI_JHD uint32_t utf8_seq_len(const uint8_t* s, uint64_t n) {
+FEI_HD uint32_t utf8_seq_len(const uint8_t* s, uint64_t n) {
   const uint32_t c = s[0];
   if (c < 0x80) return 1;
   uint32_t len, lo = 0x80, hi = 0xBF;
@@ -270,7 +258,7 @@ FEI_JHD uint32_t utf8_seq_len(const uint8_t* s, uint64_t n) {
 
 // put_json_string of a file-system name as os.fsdecode gives it: bytes that are not part of well-formed UTF-8 become the lone
 // surrogates U+DC80..U+DCFF (surrogateescape), which json.dumps writes as \udcXX.
-template <class S> FEI_JHD void put_json_fsname(S& o, const uint8_t* s, uint64_t n) {
+template <class S> FEI_HD void put_json_fsname(S& o, const uint8_t* s, uint64_t n) {
   o.put('"');
   for (uint64_t i = 0; i < n;) {
     const uint32_t len = utf8_seq_len(s + i, n - i);
@@ -288,7 +276,7 @@ template <class S> FEI_JHD void put_json_fsname(S& o, const uint8_t* s, uint64_t
   o.put('"');
 }
 
-template <class S> FEI_JHD_NI int put_value(S& o, const fei_json_col& c, uint64_t i) {
+template <class S> FEI_HD_NI int put_value(S& o, const fei_json_col& c, uint64_t i) {
   const int tag = c.tag ? c.tag[i] : c.uniform_tag;
   switch (tag) {
     case FEI_J_NULL: put_lit(o, "null"); return 0;
@@ -302,14 +290,14 @@ template <class S> FEI_JHD_NI int put_value(S& o, const fei_json_col& c, uint64_
   }
 }
 
-FEI_JHD const char* key_name(int k) {
+FEI_HD const char* key_name(int k) {
   switch (k) {
     case 0: return "difficulty"; case 1: return "index"; case 2: return "memory_id"; case 3: return "nonce"; case 4: return "previous_hash";
     case 5: return "proposer_node"; case 6: return "responsible_node"; case 7: return "solver_node"; case 8: return "task_state"; default: return "timestamp";
   }
 }
 
-template <class S> FEI_JHD_NI int put_block(S& o, const fei_json_col* cols, uint64_t i) {
+template <class S> FEI_HD_NI int put_block(S& o, const fei_json_col* cols, uint64_t i) {
   o.put('{');
   for (int k = 0; k < FEI_CHAIN_NCOLS; ++k) {
     if (k) { o.put(','); o.put(' '); }

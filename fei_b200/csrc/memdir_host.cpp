@@ -362,12 +362,12 @@ extern "C" int fei_synth_write_tree(const char* base, const char* hostname, uint
       const uint64_t k1 = k0 + 256 < n ? k0 + 256 : n;
       for (uint64_t k = k0; k < k1; ++k) {
         const uint64_t i = first + k;
-        feisynth::CountSink ch; feisynth::gen_header(ch, seed, i);
-        feisynth::CountSink cb; feisynth::gen_body(cb, seed, i);
+        fei::CountSink ch; feisynth::gen_header(ch, seed, i);
+        fei::CountSink cb; feisynth::gen_body(cb, seed, i);
         buf.resize((size_t)ch.n + 4 + cb.n);
-        { feisynth::WriteSink w(buf.data()); feisynth::gen_header(w, seed, i); }
+        { fei::WriteSink w{buf.data()}; feisynth::gen_header(w, seed, i); }
         memcpy(buf.data() + ch.n, "---\n", 4);
-        { feisynth::WriteSink w(buf.data() + ch.n + 4); feisynth::gen_body(w, seed, i); }
+        { fei::WriteSink w{buf.data() + ch.n + 4}; feisynth::gen_body(w, seed, i); }
         const feisynth::RecMeta m = feisynth::gen_meta(seed, i);
         char name[160];
         snprintf(name, sizeof(name), "%lld.%.8s.%s:2,%.*s", (long long)m.ts, m.uid, hostname, (int)m.nflags, m.flags);

@@ -16,11 +16,7 @@
 #include "jsonfmt.cuh"
 
 namespace fei {
-using feijson::CountSink;
-using feijson::WriteSink;
-using feijson::put_bytes;
 using feijson::put_json_fsname;
-using feijson::put_lit;
 
 struct RecFmtArgs {
   const uint64_t* idx; uint64_t m;                 // corpus-local records, in output order
@@ -195,13 +191,12 @@ extern "C" int fei_corpus_format_records(fei_corpus* c, const uint64_t* idx, uin
   if (!c || (m && !idx) || !out_off || (n_folders && (!folder_names || !folder_off))) { set_error("null argument"); return FEI_E_BADARG; }
   if (fmt > FEI_FMT_TEXT || (opts & ~(uint32_t)(FEI_FMT_CONTENT | FEI_FMT_SEPARATOR))) { set_error("unknown format %u / options %#x", fmt, opts); return FEI_E_BADARG; }
   std::lock_guard<std::mutex> lock(c->mu);
-  FEI_TRY(require_ready());
-  if (!c->loaded) { set_error("corpus not loaded"); return FEI_E_STATE; }
+  FEI_TRY(require_loaded(c));
   out_off[0] = 0;
   if (kernel_ms) *kernel_ms = 0.f;
   if (m == 0) return FEI_OK;
   if (!c->name.p) { set_error("the corpus was loaded without file names"); return FEI_E_STATE; }
-  for (uint64_t i = 0; i < m; ++i) if (idx[i] >= c->n) { set_error("record index %llu out of range", (unsigned long long)idx[i]); return FEI_E_BADARG; }
+  FEI_TRY(check_record_indices(c, idx, m));
   cudaStream_t s = ctx().stream;
   DevBuf d_idx, d_fold, d_fold_off, d_boff, d_body, d_len, d_off, d_out;
   FEI_TRY(upload(d_idx, idx, m * 8, 0, s));
@@ -210,15 +205,18 @@ extern "C" int fei_corpus_format_records(fei_corpus* c, const uint64_t* idx, uin
   struct Events { cudaEvent_t e[2] = {nullptr, nullptr}; ~Events() { for (auto x : e) if (x) cudaEventDestroy(x); } } ev;
   for (auto& e : ev.e) FEI_CUDA(cudaEventCreate(&e));
   FEI_CUDA(cudaEventRecord(ev.e[0], s));
-  if (opts & FEI_FMT_CONTENT) FEI_TRY(untile_bodies(c, d_idx.as<uint64_t>(), m, d_boff, d_body, s));
+  if (opts & FEI_FMT_CONTENT) {
+    uint64_t bytes = 0;
+    FEI_TRY(fetch_offsets(c, d_idx.as<uint64_t>(), 0, m, nullptr, d_boff, nullptr, &bytes, false, s));
+    FEI_TRY(untile_bodies(c, d_idx.as<uint64_t>(), 0, m, d_boff, bytes, d_body, s));
+  }
   const RecFmtArgs a{d_idx.as<uint64_t>(), m, c->hdr.as<uint8_t>(), c->hdr_off.as<uint64_t>(), c->name.as<uint8_t>(), c->name_off.as<uint64_t>(),
                      c->name_spans.as<uint16_t>(), c->ts.as<int64_t>(), c->wall.as<int64_t>(), c->flags8.as<uint64_t>(), c->fsb.as<uint32_t>(),
                      d_body.as<uint8_t>(), d_boff.as<uint64_t>(), d_fold.as<uint8_t>(), d_fold_off.as<uint64_t>(), n_folders, fmt, opts};
   FEI_TRY(d_len.alloc(m * 4)); FEI_TRY(d_off.alloc((m + 1) * 8));
   const unsigned grid = (unsigned)((m + 127) / 128);
   k_recfmt_measure<<<grid, 128, 0, s>>>(a, d_len.as<uint32_t>());
-  FEI_TRY(exclusive_scan_u32_u64(d_len.as<uint32_t>(), m, d_off.as<uint64_t>(), c->scan_tmp, s));
-  FEI_CUDA(cudaMemcpyAsync(out_off, d_off.p, (m + 1) * 8, cudaMemcpyDeviceToHost, s));
+  FEI_TRY(queue_offsets(d_len.as<uint32_t>(), m, d_off.as<uint64_t>(), out_off, true, c->scan_tmp, s));
   FEI_CUDA(cudaStreamSynchronize(s));
   FEI_CUDA(cudaGetLastError());
   const uint64_t total = out_off[m];

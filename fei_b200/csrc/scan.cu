@@ -35,6 +35,7 @@
 #include "../../include/feiscan_prog.h"
 #include "pyws.cuh"
 #include "datefmt.cuh"
+#include "sink.cuh"
 #include <string.h>
 #include <stdlib.h>
 #include <vector>
@@ -1939,10 +1940,17 @@ static int check_prog(const uint8_t* prog, uint64_t len) {
 enum { kCompactNone = kScanCompactNone, kCompactLists = kScanCompactLists };
 constexpr int kWorkCounters = 6;           // work_counter: [0] = BodyArgs::next, [2] = header survivors, the rest see BodyArgs::counter
 
+// key_lut for the program already in c->prog, queued on s: which of the program's fields each distinct header key of the corpus names
+static int build_key_lut(fei_corpus* c, cudaStream_t s) {
+  FEI_TRY(c->key_lut.ensure(kKeySlots * sizeof(uint32_t)));
+  k_key_lut<<<kKeySlots / 128, 128, 0, s>>>(c->prog.as<uint8_t>(), c->hdr.as<uint8_t>(), c->key_tag.as<unsigned long long>(),
+                                            c->key_rep.as<unsigned long long>(), c->key_len.as<uint32_t>(), c->key_lut.as<uint32_t>());
+  return FEI_OK;
+}
+
 // Everything is queued on the context stream; nothing here waits for the GPU.
 int run_scan(fei_corpus* c, const uint8_t* prog, uint64_t prog_len, int compact_mode, ScanHook* hook) {
-  FEI_TRY(require_ready());
-  if (!c || !c->loaded) { set_error("corpus not loaded"); return FEI_E_STATE; }
+  FEI_TRY(require_loaded(c));
   FEI_TRY(check_prog(prog, prog_len));
   Context& cx = ctx();
   cudaStream_t s = cx.stream;
@@ -2001,11 +2009,9 @@ int run_scan(fei_corpus* c, const uint8_t* prog, uint64_t prog_len, int compact_
         }
       for (int x = 0; x < FEI_MAX_AUX; ++x) a.aux[x] = c->aux[x].as<uint8_t>();
     }
-    if (h.n_slots) {                                           // which of the program's fields does each distinct header key of the corpus name?
-      FEI_TRY(c->key_lut.ensure(kKeySlots * sizeof(uint32_t)));
+    if (h.n_slots) {
+      FEI_TRY(build_key_lut(c, s));
       a.key_lut = c->key_lut.as<uint32_t>();
-      k_key_lut<<<kKeySlots / 128, 128, 0, s>>>(c->prog.as<uint8_t>(), c->hdr.as<uint8_t>(), c->key_tag.as<unsigned long long>(),
-                                                c->key_rep.as<unsigned long long>(), c->key_len.as<uint32_t>(), c->key_lut.as<uint32_t>());
       FEI_TRY(c->slot_col.ensure(FEI_MAX_SLOTS));
       FEI_TRY(c->kid_col.ensure(kKeySlots));
       a.slot_col = c->slot_col.as<int8_t>();
@@ -2498,8 +2504,7 @@ extern "C" int fei_corpus_slot_values(fei_corpus* c, const uint8_t* prog, uint64
                                       uint8_t* blob, uint64_t blob_cap) {
   if (!c || !prog || !present || !off) { set_error("null argument"); return FEI_E_BADARG; }
   std::lock_guard<std::mutex> lock(c->mu);
-  FEI_TRY(require_ready());
-  if (!c->loaded) { set_error("corpus not loaded"); return FEI_E_STATE; }
+  FEI_TRY(require_loaded(c));
   FEI_TRY(check_prog(prog, prog_len));
   fei_prog_hdr h; memcpy(&h, prog, sizeof(h));
   if (h.n_slots < 1) { set_error("program has no header field"); return FEI_E_BADARG; }
@@ -2509,17 +2514,14 @@ extern "C" int fei_corpus_slot_values(fei_corpus* c, const uint8_t* prog, uint64
   cudaStream_t s = ctx().stream;
   FEI_TRY(c->prog.ensure(prog_len + 16));
   FEI_CUDA(cudaMemcpyAsync(c->prog.p, prog, prog_len, cudaMemcpyHostToDevice, s));
-  FEI_TRY(c->key_lut.ensure(kKeySlots * sizeof(uint32_t)));
-  k_key_lut<<<kKeySlots / 128, 128, 0, s>>>(c->prog.as<uint8_t>(), c->hdr.as<uint8_t>(), c->key_tag.as<unsigned long long>(),
-                                            c->key_rep.as<unsigned long long>(), c->key_len.as<uint32_t>(), c->key_lut.as<uint32_t>());
+  FEI_TRY(build_key_lut(c, s));
   HeadArgs a{c->prog.as<uint8_t>(), c->hdr.as<uint8_t>(), c->hdr_off.as<uint64_t>(), nullptr, nullptr, nullptr, c->wall.as<int64_t>(), c->flags8.as<uint64_t>(),
              c->fsb.as<uint32_t>(), n, nullptr, c->hdir.as<uint2>(), c->hdir_off.as<uint64_t>(), c->key_lut.as<uint32_t>(), false, nullptr, nullptr, nullptr, c->ts.as<int64_t>(), {}};
   DevBuf d_len, d_src, d_off, d_present, d_out;
   FEI_TRY(d_len.alloc(n * 4)); FEI_TRY(d_src.alloc(n * 8)); FEI_TRY(d_off.alloc((n + 1) * 8)); FEI_TRY(d_present.alloc(n));
   const unsigned grid = (unsigned)((n + 255) / 256);
   k_slot_spans<<<grid, 256, 0, s>>>(a, d_len.as<uint32_t>(), d_src.as<uint64_t>());
-  FEI_TRY(exclusive_scan_u32_u64(d_len.as<uint32_t>(), n, d_off.as<uint64_t>(), c->scan_tmp, s));
-  FEI_CUDA(cudaMemcpyAsync(off, d_off.p, (n + 1) * 8, cudaMemcpyDeviceToHost, s));
+  FEI_TRY(queue_offsets(d_len.as<uint32_t>(), n, d_off.as<uint64_t>(), off, true, c->scan_tmp, s));
   FEI_CUDA(cudaStreamSynchronize(s));
   FEI_TRY(d_out.alloc(off[n] + 16));
   k_slot_gather<<<grid, 256, 0, s>>>(c->hdr.as<uint8_t>(), d_len.as<uint32_t>(), d_src.as<uint64_t>(), d_off.as<uint64_t>(), n, d_out.as<uint8_t>(), d_present.as<uint8_t>());
@@ -2644,8 +2646,6 @@ __device__ __forceinline__ bool tag_edit_changes(const TagOps& o, const TagRecor
   return false;
 }
 
-struct CountSink { uint32_t n = 0; __device__ void put(const uint8_t*, uint32_t l) { n += l; } };
-struct CopySink { uint8_t* d; __device__ void put(const uint8_t* p, uint32_t l) { for (uint32_t k = 0; k < l; ++k) *d++ = p[k]; } };
 template <class Sink>
 struct Joiner {                                                  // ", ".join
   Sink& s; bool first = true;
@@ -2706,12 +2706,12 @@ __global__ void __launch_bounds__(256) k_tag_edit_write(TagEditArgs a, const uin
   if (rec >= a.n || !changed[rec]) return;
   const TagRecord r = tag_record(a, rec);
   const uint64_t j = pos[rec], o = off[rec];
-  CopySink s{text + o};
+  WriteSink s{text + o};
   if (r.has_subj) s.put(r.subj, r.subj_len);
   text_off[3 * j] = o;
-  text_off[3 * j + 1] = o + (uint64_t)(s.d - (text + o));
+  text_off[3 * j + 1] = o + (uint64_t)(s.p - (text + o));
   emit_old_tags(s, r);
-  text_off[3 * j + 2] = o + (uint64_t)(s.d - (text + o));
+  text_off[3 * j + 2] = o + (uint64_t)(s.p - (text + o));
   emit_new_tags(s, ops, r);
   rec_out[j] = rec + global_base;
   has_subject[j] = r.has_subj ? 1 : 0;
@@ -2756,11 +2756,9 @@ extern "C" int fei_corpus_tag_edit(fei_corpus* c, const uint8_t* prog, uint64_t 
                       c->key_lut.as<uint32_t>(), c->hits.as<uint32_t>(), n, d_ops.as<TagOps>()};
   const unsigned grid = (unsigned)((n + 255) / 256);
   k_tag_edit_measure<<<grid, 256, 0, s>>>(a, d_changed.as<uint32_t>(), d_bytes.as<uint32_t>());
-  FEI_TRY(exclusive_scan_u32_u64(d_changed.as<uint32_t>(), n, d_pos.as<uint64_t>(), c->scan_tmp, s));
-  FEI_TRY(exclusive_scan_u32_u64(d_bytes.as<uint32_t>(), n, d_off.as<uint64_t>(), c->scan_tmp, s));
   uint64_t count = 0, total = 0;
-  FEI_CUDA(cudaMemcpyAsync(&count, d_pos.as<uint64_t>() + n, 8, cudaMemcpyDeviceToHost, s));
-  FEI_CUDA(cudaMemcpyAsync(&total, d_off.as<uint64_t>() + n, 8, cudaMemcpyDeviceToHost, s));
+  FEI_TRY(queue_offsets(d_changed.as<uint32_t>(), n, d_pos.as<uint64_t>(), &count, false, c->scan_tmp, s));
+  FEI_TRY(queue_offsets(d_bytes.as<uint32_t>(), n, d_off.as<uint64_t>(), &total, false, c->scan_tmp, s));
   FEI_CUDA(cudaStreamSynchronize(s));
   if (count > cap || total > text_cap || (count && (!rec || !text || !has_subject))) {
     *n_changed = count; text_off[0] = total;

@@ -62,8 +62,7 @@ using namespace fei;
 extern "C" int fei_corpus_save(fei_corpus* c, const char* path) {
   if (!c || !path) { set_error("null argument"); return FEI_E_BADARG; }
   std::lock_guard<std::mutex> lock(c->mu);
-  FEI_TRY(require_ready());
-  if (!c->loaded) { set_error("corpus not loaded"); return FEI_E_STATE; }
+  FEI_TRY(require_loaded(c));
   cudaStream_t s = ctx().copy_stream;
   const int fd = open(path, O_WRONLY | O_CREAT | O_TRUNC, 0644);
   if (fd < 0) { set_error("open(%s): %s", path, strerror(errno)); return FEI_E_BADARG; }

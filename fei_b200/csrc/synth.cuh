@@ -15,16 +15,10 @@
 //   body = text after the separator, already .strip()ped (utils.py:120)
 #pragma once
 #include <stdint.h>
-
-#if defined(__CUDACC__)
-#define FEI_HD __host__ __device__ __forceinline__
-#define FEI_HD_NOINLINE __host__ __device__
-#else
-#define FEI_HD inline
-#define FEI_HD_NOINLINE
-#endif
+#include "sink.cuh"
 
 namespace feisynth {
+using fei::put_lit;
 
 struct Word { uint8_t len; char s[55]; };
 #define FW(x) { (uint8_t)(sizeof(x) - 1), x }
@@ -130,19 +124,7 @@ struct Rng {
   FEI_HD bool chance(uint32_t pct) { return below(100) < pct; }
 };
 
-// ---------------------------------------------------------------- sinks
-struct CountSink {
-  uint32_t n;
-  FEI_HD CountSink() : n(0) {}
-  FEI_HD void put(char) { ++n; }
-};
-struct WriteSink {
-  uint8_t* p; uint32_t n;
-  FEI_HD explicit WriteSink(uint8_t* dst) : p(dst), n(0) {}
-  FEI_HD void put(char c) { p[n++] = (uint8_t)c; }
-};
-
-template <class S> FEI_HD void put_lit(S& s, const char* z) { while (*z) s.put(*z++); }
+// ---------------------------------------------------------------- writers (into a sink.cuh sink)
 template <class S> FEI_HD void put_word(S& s, int wi) { const Word& w = word(wi); for (int k = 0; k < w.len; ++k) s.put(w.s[k]); }
 template <class S> FEI_HD void put_word_lower(S& s, int wi, bool cap_first) {
   const Word& w = word(wi);

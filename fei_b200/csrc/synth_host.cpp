@@ -60,13 +60,13 @@ extern "C" int fei_synth_record_host(uint64_t seed, uint64_t i,
                                      uint8_t* body, uint32_t body_cap, uint32_t* body_len,
                                      int64_t* ts, char* uid8, char* flags4, uint8_t* nflags, uint8_t* status, uint8_t* folder) {
   using namespace feisynth;
-  CountSink ch; gen_header(ch, seed, i);
-  CountSink cb; gen_body(cb, seed, i);
+  fei::CountSink ch; gen_header(ch, seed, i);
+  fei::CountSink cb; gen_body(cb, seed, i);
   if (hdr_len) *hdr_len = ch.n;
   if (body_len) *body_len = cb.n;
   if ((hdr && ch.n > hdr_cap) || (body && cb.n > body_cap)) { fei::set_error("record %llu needs %u header / %u body bytes", (unsigned long long)i, ch.n, cb.n); return FEI_E_CAPACITY; }
-  if (hdr) { WriteSink w(hdr); gen_header(w, seed, i); }
-  if (body) { WriteSink w(body); gen_body(w, seed, i); }
+  if (hdr) { fei::WriteSink w{hdr}; gen_header(w, seed, i); }
+  if (body) { fei::WriteSink w{body}; gen_body(w, seed, i); }
   RecMeta m = gen_meta(seed, i);
   if (ts) *ts = m.ts;
   if (uid8) memcpy(uid8, m.uid, 8);
