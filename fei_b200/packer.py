@@ -31,7 +31,7 @@ import struct
 import threading
 import time
 from datetime import datetime
-from typing import Any, Dict, Iterator, List, Optional, Sequence, Tuple
+from typing import Any, Callable, Dict, Iterator, List, Optional, Sequence, Tuple
 
 import numpy as np
 
@@ -48,6 +48,7 @@ FORMAT_CHUNK_BYTES = 64 << 20                                      # formatted o
 LIST_CONCURRENCY = 4                                                # directories listed at the same time in a cold pack
 READ_THREADS = max(1, min(32, len(os.sched_getaffinity(0)) if hasattr(os, "sched_getaffinity") else (os.cpu_count() or 1)))
 _KEY_DT = np.dtype([("ino", "u8"), ("size", "u8"), ("mtime", "i8")])
+_META_COLS = {"ts": np.int64, "wall": np.int64, "flags8": np.uint64, "fsb": np.uint32}   # per-record meta columns (fsb: folder | status << 16 | record bits << 24)
 
 
 # ----------------------------------------------------------------------------- native directory listing
@@ -67,11 +68,36 @@ class DirListing:
         k["ino"], k["size"], k["mtime"] = self.ino, self.size, self.mtime_ns
         return k
 
+    def ident(self, i: int) -> Tuple[int, int, int]:
+        """key()[i] as (inode, size, mtime)."""
+        return int(self.ino[i]), int(self.size[i]), int(self.mtime_ns[i])
+
 
 def _arr(p, dt, k):
     if not k:
         return np.zeros(0, dtype=dt)
     return np.ctypeslib.as_array(C.cast(p, C.POINTER(np.ctypeslib.as_ctypes_type(dt))), shape=(k,)).copy()
+
+
+def _cat(parts: Sequence[np.ndarray], dtype, *shape: int) -> np.ndarray:
+    """np.concatenate that also takes no parts (then an empty array of `dtype` whose rows have `shape`)."""
+    return np.concatenate(parts) if parts else np.zeros((0, *shape), dtype=dtype)
+
+
+def _offsets(lengths) -> np.ndarray:
+    """off[k + 1] (uint64) with off[0] = 0 and off[i + 1] - off[i] = lengths[i]."""
+    off = np.zeros(len(lengths) + 1, dtype=np.uint64)
+    np.cumsum(lengths, out=off[1:])
+    return off
+
+
+def _take_names(names: bytes, name_off: np.ndarray, sel) -> Tuple[bytes, np.ndarray]:
+    """Entries `sel` (indices, or a slice for a contiguous range) of a names blob + offsets: (their blob, their offsets from 0)."""
+    if isinstance(sel, slice):
+        lo, hi, _ = sel.indices(len(name_off) - 1)
+        a = name_off[lo]
+        return names[int(a):int(name_off[hi])], name_off[lo:hi + 1] - a
+    return b"".join(names[int(name_off[i]):int(name_off[i + 1])] for i in sel.tolist()), _offsets(np.diff(name_off)[sel])
 
 
 def list_dir(path: str, want_stat: bool = True) -> DirListing:
@@ -121,13 +147,7 @@ def list_dir(path: str, want_stat: bool = True) -> DirListing:
         except Exception as e:                                        # reported like the reference reports a bad file (utils.py:247-248)
             d.bad.append(f"Error processing {name}: {e}")
     idx = np.nonzero(keep)[0]
-    lens = (name_off[1:] - name_off[:-1]).astype(np.int64)
-    if len(idx) == n:
-        d.names, d.name_off = blob, name_off
-    else:
-        d.names = b"".join(blob[int(name_off[i]):int(name_off[i + 1])] for i in idx.tolist())
-        d.name_off = np.zeros(len(idx) + 1, dtype=np.uint64)
-        np.cumsum(lens[idx], out=d.name_off[1:])
+    d.names, d.name_off = (blob, name_off) if len(idx) == n else _take_names(blob, name_off, idx)
     for k, a in cols.items():
         setattr(d, k, a[idx])
     d.spans = spans[idx]
@@ -145,43 +165,17 @@ def list_dir(path: str, want_stat: bool = True) -> DirListing:
     return d
 
 
-def read_range_into(path: str, d: DirListing, lo: int, hi: int, out: np.ndarray) -> bool:
-    """Entries [lo, hi) of the listing read back to back into out[0 : sum(sizes)] (native threads).  False if any file could not
-    be read or no longer has its listed size (the caller then takes the careful path)."""
-    k = hi - lo
-    if k <= 0:
-        return True
-    a, b = int(d.name_off[lo]), int(d.name_off[hi])
-    nbuf = np.frombuffer(d.names, dtype=np.uint8)[a:b] if b > a else np.zeros(1, dtype=np.uint8)
-    name_off = np.ascontiguousarray(d.name_off[lo:hi + 1] - np.uint64(a))
-    sizes = d.size[lo:hi]
-    off = np.zeros(k + 1, dtype=np.uint64)
-    np.cumsum(sizes, out=off[1:])
-    got = np.zeros(k, dtype=np.uint64); err = np.zeros(k, dtype=np.int32)
-    _abi.check(_abi.lib().fei_read_files(os.fsencode(path), nbuf.ctypes.data, _abi.ptr(name_off), k, out.ctypes.data, _abi.ptr(off), READ_THREADS,
-                                        _abi.ptr(got), _abi.ptr(err)))
-    return not err.any() and bool((got == sizes).all())
-
-
-def read_files(path: str, d: DirListing, sel: Optional[np.ndarray] = None, out: Optional[np.ndarray] = None, out_base: int = 0
+def read_files(path: str, d: DirListing, sel=None, out: Optional[np.ndarray] = None, out_base: int = 0, retry: bool = True
                ) -> Tuple[np.ndarray, np.ndarray, List[Tuple[int, str]]]:
-    """Contents of the selected entries (all when sel is None): (raw blob, offsets[k+1], [(k, error message)]).  With `out`, the
-    bytes land in out[out_base : out_base + sum(sizes)] (one buffer for a whole tree, no concatenation afterwards)."""
-    if sel is None:
-        names, name_off, sizes = d.names, d.name_off, d.size
-    else:
-        sel = np.asarray(sel, dtype=np.int64)
-        names = b"".join(d.name_bytes(i) for i in sel.tolist())
-        name_off = np.zeros(len(sel) + 1, dtype=np.uint64)
-        np.cumsum((d.name_off[1:] - d.name_off[:-1])[sel], out=name_off[1:])
-        sizes = d.size[sel]
+    """Contents of the selected entries (all when sel is None; indices, or a slice for a contiguous range), read by native threads:
+    (raw blob, offsets[k+1], [(k, error message)]).  With `out`, the bytes land in out[out_base : out_base + sum(sizes)] (one
+    buffer for a whole tree or a reused chunk buffer, no concatenation afterwards).  A file that could not be read or no longer
+    has its listed size is read again on its own; with retry=False it is only reported (the caller then takes the careful path)."""
+    names, name_off = (d.names, d.name_off) if sel is None else _take_names(d.names, d.name_off, sel)
+    sizes = d.size if sel is None else d.size[sel]
     k = len(sizes)
-    off = np.zeros(k + 1, dtype=np.uint64)
-    np.cumsum(sizes, out=off[1:])
-    if out is None:
-        raw = np.empty(max(1, int(off[k])), dtype=np.uint8)
-    else:
-        raw = out[out_base:out_base + max(1, int(off[k]))]
+    off = _offsets(sizes)
+    raw = np.empty(max(1, int(off[k])), dtype=np.uint8) if out is None else out[out_base:out_base + max(1, int(off[k]))]
     got = np.zeros(max(1, k), dtype=np.uint64)
     err = np.zeros(max(1, k), dtype=np.int32)
     nbuf = np.frombuffer(names, dtype=np.uint8) if names else np.zeros(1, dtype=np.uint8)
@@ -189,18 +183,20 @@ def read_files(path: str, d: DirListing, sel: Optional[np.ndarray] = None, out: 
                                         READ_THREADS, _abi.ptr(got), _abi.ptr(err)))
     problems: List[Tuple[int, str]] = []
     short = np.nonzero((err[:k] != 0) | (got[:k] != sizes))[0]
+    name_of = lambda i: os.fsdecode(names[int(name_off[i]):int(name_off[i + 1])])
+    if len(short) and not retry:
+        return raw, off, [(i, f"Error processing {name_of(i)}: changed or vanished since it was listed") for i in short.tolist()]
     if len(short):                                                    # shrunk or vanished between stat and read: read those again, one by one
         parts = [raw[int(off[i]):int(off[i + 1])].tobytes() for i in range(k)]
         for i in short.tolist():
-            name = os.fsdecode(names[int(name_off[i]):int(name_off[i + 1])])
+            name = name_of(i)
             try:
                 with open(os.path.join(path, name), "rb") as f:
                     parts[i] = f.read()
             except OSError as e:
                 parts[i] = b""
                 problems.append((i, f"Error processing {name}: {e}"))
-        off = np.zeros(k + 1, dtype=np.uint64)
-        np.cumsum(np.fromiter(map(len, parts), dtype=np.int64, count=k), out=off[1:])
+        off = _offsets(np.fromiter(map(len, parts), dtype=np.int64, count=k))
         raw = np.frombuffer(b"".join(parts), dtype=np.uint8).copy() if off[k] else np.zeros(1, dtype=np.uint8)
         if out is not None and int(off[k]) <= len(out) - out_base:      # keep the one-buffer layout when it still fits
             out[out_base:out_base + int(off[k])] = raw[:int(off[k])]
@@ -373,6 +369,62 @@ class _Seg:
     __slots__ = ("listing", "dev", "mtime_ns", "bad", "bad_files")      # bad_files: name -> (inode, size, mtime) of files that could not be packed
 
 
+def _new_seg(listing: DirListing, mtime_ns: int, dev_fill: int) -> _Seg:
+    seg = _Seg()
+    seg.listing, seg.mtime_ns, seg.dev, seg.bad, seg.bad_files = listing, mtime_ns, np.full(listing.n, dev_fill, dtype=np.int64), list(listing.bad), {}
+    return seg
+
+
+def _report_unpackable(seg: _Seg, i: int, blob: bytes) -> None:
+    """Entry i holds `blob`, which is not UTF-8: reported and skipped like the reference (utils.py:247-248), and remembered by
+    (inode, size, mtime) so that later syncs keep it out without reading it again while it does not change."""
+    L = seg.listing
+    seg.bad.append(f"Error processing {L.name(i)}: {_decode_error(blob)}")
+    seg.bad_files[L.name_bytes(i)] = L.ident(i)
+
+
+class _Stager:
+    """Sends pieces of a cold pack's text to their place in the device text (Corpus.stage_text, a pageable copy) from a side
+    thread, in the order they were put, while the caller reads the next piece.  After a failure the remaining pieces are skipped;
+    `consumed(tag)` runs after each piece, once stage_text has returned and the piece's host bytes may be reused."""
+
+    def __init__(self, corpus, total: int, consumed: Optional[Callable[[Any], None]] = None):
+        self.failed: List[BaseException] = []
+        self._jobs: "queue.Queue[Optional[Tuple[np.ndarray, int, Any]]]" = queue.Queue()
+        self._thread = threading.Thread(target=self._run, args=(corpus, total, consumed), daemon=True)
+        self._thread.start()
+
+    def _run(self, corpus, total: int, consumed) -> None:
+        while (job := self._jobs.get()) is not None:
+            piece, offset, tag = job
+            if not self.failed:
+                try:
+                    corpus.stage_text(total, piece, offset)             # returns once the pageable source has been consumed
+                except BaseException as e:                              # noqa: BLE001 -- the caller falls back to a path that does not stage
+                    self.failed.append(e)
+            if consumed is not None:
+                consumed(tag)
+
+    def put(self, piece: np.ndarray, offset: int, tag: Any = None) -> None:
+        self._jobs.put((piece, offset, tag))
+
+    def close(self) -> None:
+        """Returns once every piece put so far has been consumed."""
+        self._jobs.put(None)
+        self._thread.join()
+
+
+def _load_arrays(names: bytes, name_off: np.ndarray, spans, cols: Dict[str, Any], **text) -> Dict[str, Any]:
+    """What Corpus.load_raw takes: records in listing order (names blob + offsets, name spans, the _META_COLS) plus their text,
+    given either as raw + raw_begin + raw_len + raw_bytes (fei_corpus_load_raw_spans; raw None = already staged on the device) or
+    as raw + raw_off (fei_corpus_load_raw)."""
+    n = len(cols["ts"])
+    return {"n": n, "global_base": 0, **text,
+            "name": (np.frombuffer(names, dtype=np.uint8).copy() if names else np.zeros(1, dtype=np.uint8)) if n else None,
+            "name_off": name_off if n else None, "name_spans": np.ascontiguousarray(spans, dtype=np.uint16).reshape(-1) if n else None,
+            **{k: np.ascontiguousarray(cols[k], dtype=dt) for k, dt in _META_COLS.items()}}
+
+
 def _headers_of(text: str) -> Dict[str, str]:
     headers: Dict[str, str] = {}
     for line in text.strip().split("\n"):
@@ -535,6 +587,14 @@ class PackedMemdir:
             mt = -1
         return list_dir(path, want_stat), mt
 
+    def _list_many(self, keys: List[Tuple[str, str]]) -> List[Tuple[DirListing, int]]:
+        """_list of several directories, LIST_CONCURRENCY at a time: readdir is serial per directory."""
+        if len(keys) < 2:
+            return [self._list(*k) for k in keys]
+        from concurrent.futures import ThreadPoolExecutor
+        with ThreadPoolExecutor(min(LIST_CONCURRENCY, len(keys))) as ex:
+            return list(ex.map(lambda k: self._list(*k), keys))
+
     def _fsb_of(self, key: Tuple[str, str]) -> int:
         return (self.folder_ids[key[0]] & 0xFFFF) | (U.STANDARD_FOLDERS.index(key[1]) << 16)
 
@@ -597,17 +657,15 @@ class PackedMemdir:
                 for j in alive[~valid].tolist():                       # undecodable files: reported and skipped (utils.py:247-248)
                     keep[j] = False
                     key, i = self._locate(segs, order, j)
-                    L = segs[key].listing
                     if raw is not None:
                         blob = raw[int(begin[j]):int(begin[j] + ln[j])].tobytes()
                     else:                                              # the text only exists on the device: read this one file again for the message
                         try:
-                            with open(os.path.join(self._dir(*key), L.name(i)), "rb") as f:
+                            with open(os.path.join(self._dir(*key), segs[key].listing.name(i)), "rb") as f:
                                 blob = f.read()
                         except OSError:
                             blob = b"\xff"
-                    segs[key].bad.append(f"Error processing {L.name(i)}: {_decode_error(blob)}")
-                    segs[key].bad_files[L.name_bytes(i)] = (int(L.ino[i]), int(L.size[i]), int(L.mtime_ns[i]))
+                    _report_unpackable(segs[key], i, blob)
             raw_bytes = int(ln.sum())
         finally:
             tf = time.perf_counter()
@@ -660,8 +718,7 @@ class PackedMemdir:
                 t = time.perf_counter()
                 listing, mt = fut.result()
                 fut = ex.submit(self._list, *order[k + 1], want_stat=False) if k + 1 < len(order) else None
-                seg = _Seg(); seg.listing = listing; seg.mtime_ns = mt; seg.bad = list(listing.bad); seg.bad_files = {}; seg.dev = np.zeros(listing.n, dtype=np.int64)
-                segs[key] = seg
+                segs[key] = _new_seg(listing, mt, 0)
                 t1 = time.perf_counter(); t_list += t1 - t
                 if listing.n:
                     b, l, e = read_dir_packed(self._dir(*key), listing, arena)
@@ -673,9 +730,8 @@ class PackedMemdir:
             raise NotImplementedError("tree larger than one packing batch; shard it over several corpora")
         t = time.perf_counter()
         arena.pin_finished(final=True)
-        cat = lambda xs, dt: np.concatenate(xs) if xs else np.zeros(0, dtype=dt)
         self.timing = {"list_s": t_list, "read_s": t_read, "pin_tail_s": time.perf_counter() - t, "cold_path": "names-only listing (of the next directory, under the current read), open+fstat+read+close into an arena; list_s = listing time not hidden"}
-        return arena.buf[:max(1, total)], cat(begins, np.uint64), cat(lens, np.uint64), cat(errs, np.int32)
+        return arena.buf[:max(1, total)], _cat(begins, np.uint64), _cat(lens, np.uint64), _cat(errs, np.int32)
 
     def _cold_read_listed(self, order, segs, corpus=None):
         """The default cold read: a listing with a stat of every entry (sizes known), then the files are read CHUNK by CHUNK into a
@@ -685,12 +741,8 @@ class PackedMemdir:
         to the one-buffer path below."""
         t0 = time.perf_counter()
         total = 0
-        from concurrent.futures import ThreadPoolExecutor
-        with ThreadPoolExecutor(max(1, min(LIST_CONCURRENCY, len(order)))) as ex:   # 1. list every directory (readdir + parallel stat, native):
-            listed = list(ex.map(lambda k: self._list(*k), order))                  #    readdir is serial per directory, so several at a time
-        for key, (listing, mt) in zip(order, listed):
-            seg = _Seg(); seg.listing = listing; seg.mtime_ns = mt; seg.bad = list(listing.bad); seg.bad_files = {}; seg.dev = np.zeros(listing.n, dtype=np.int64)
-            segs[key] = seg
+        for key, (listing, mt) in zip(order, self._list_many(order)):  # 1. list every directory (readdir + parallel stat, native)
+            segs[key] = _new_seg(listing, mt, 0)
             total += int(listing.size.sum())
         if total > MAX_RAW_BATCH:
             raise NotImplementedError("tree larger than one packing batch; shard it over several corpora")
@@ -716,63 +768,41 @@ class PackedMemdir:
         free: "queue.Queue[int]" = queue.Queue()
         for k in range(COLD_SLOTS):
             free.put(k)
-        jobs: "queue.Queue[Optional[Tuple[int, int, int]]]" = queue.Queue()
-        failed: List[BaseException] = []
-
-        def uploader():
-            while True:
-                job = jobs.get()
-                if job is None:
-                    return
-                slot, offset, nbytes = job
-                if not failed:
-                    try:
-                        corpus.stage_text(total, slots[slot].buf[:nbytes], offset)     # returns once the pageable source has been consumed
-                    except BaseException as e:                          # noqa: BLE001 -- the caller falls back to the one-buffer path
-                        failed.append(e)
-                free.put(slot)
-        th = threading.Thread(target=uploader, daemon=True)
-        th.start()
+        stager = _Stager(corpus, total, consumed=free.put)             # a slot is free again once its chunk has been staged
         ok = True
         base_off = 0
-        sizes_all = []
         try:
             for key in order:
                 L = segs[key].listing
                 if not L.n:
                     continue
-                sizes_all.append(L.size)
-                cs = np.zeros(L.n + 1, dtype=np.int64)
-                np.cumsum(L.size.astype(np.int64), out=cs[1:])
+                cs = _offsets(L.size).astype(np.int64)
                 lo = 0
-                while lo < L.n and ok and not failed:
+                while lo < L.n and ok and not stager.failed:
                     hi = int(np.searchsorted(cs, cs[lo] + COLD_CHUNK_BYTES, side="right")) - 1
                     hi = min(L.n, max(hi, lo + 1))
                     slot = free.get()
                     nbytes = int(cs[hi] - cs[lo])
-                    ok = read_range_into(self._dir(*key), L, lo, hi, slots[slot].buf)
+                    ok = not read_files(self._dir(*key), L, slice(lo, hi), out=slots[slot].buf, retry=False)[2]
                     if not ok:
                         free.put(slot)
                         break
-                    jobs.put((slot, base_off + int(cs[lo]), nbytes))
+                    stager.put(slots[slot].buf[:nbytes], base_off + int(cs[lo]), slot)
                     lo = hi
-                if not ok or failed:
+                if not ok or stager.failed:
                     break
                 base_off += int(cs[L.n])
         finally:
             t_reads_done = time.perf_counter()
-            jobs.put(None)
-            th.join()
+            stager.close()
             tf = time.perf_counter()
             for sl in slots:
                 sl.close()
             t_freed = time.perf_counter()
-        if not ok or failed or base_off != total:
+        if not ok or stager.failed or base_off != total:
             return None
-        sizes = np.concatenate(sizes_all).astype(np.uint64) if sizes_all else np.zeros(0, dtype=np.uint64)
-        begin = np.zeros(n, dtype=np.uint64)
-        if n > 1:
-            np.cumsum(sizes[:-1], out=begin[1:])
+        sizes = _cat([segs[key].listing.size for key in order], np.uint64)
+        begin = _offsets(sizes)[:-1]
         self._cold_total = total
         self.timing = {"read_s": t_reads_done - t1, "upload_tail_s": tf - t_reads_done, "free_chunk_buffers_s": t_freed - tf,
                        "cold_path": "listing with stat; files read in %d MiB chunks into %d reused host buffers, each chunk uploaded under the next read" % (COLD_CHUNK_BYTES >> 20, COLD_SLOTS)}
@@ -790,22 +820,7 @@ class PackedMemdir:
         pos = base_off = 0
         exact = True
         stage = corpus is not None and total > 0 and os.environ.get("FEI_STAGE_UPLOAD", "1") != "0"
-        jobs: "queue.Queue[Optional[Tuple[int, int]]]" = queue.Queue()
-        failed: List[BaseException] = []
-
-        def uploader():
-            while True:
-                job = jobs.get()
-                if job is None:
-                    return
-                if not failed:
-                    try:
-                        corpus.stage_text(total, raw[job[0]:job[1]], job[0])
-                    except BaseException as e:                          # noqa: BLE001 -- reported by falling back to the plain upload
-                        failed.append(e)
-        th = threading.Thread(target=uploader, daemon=True) if stage else None
-        if th:
-            th.start()
+        stager = _Stager(corpus, total) if stage else None             # a failed staging falls back to the plain upload from `raw`
         try:
             for key in order:
                 L = segs[key].listing
@@ -818,18 +833,17 @@ class PackedMemdir:
                     pieces = [raw[:base_off].copy()]
                 if not exact:
                     pieces.append(r[:int(off[-1])].copy())
-                elif th:
-                    jobs.put((base_off, base_off + int(off[-1])))
+                elif stager:
+                    stager.put(raw[base_off:base_off + int(off[-1])], base_off)
                 raw_off[pos + 1:pos + L.n + 1] = off[1:] + np.uint64(base_off)
                 pos += L.n; base_off += int(off[-1])
         finally:
             t_reads_done = time.perf_counter()
-            if th:
-                jobs.put(None)
-                th.join()
+            if stager:
+                stager.close()
         if not exact:
             raw = np.concatenate(pieces) if pieces else np.zeros(1, dtype=np.uint8)
-        staged = bool(th) and exact and not failed and base_off == total
+        staged = stager is not None and exact and not stager.failed and base_off == total
         self.timing = {"list_s": t1 - t0, "read_s": t_reads_done - t1, "upload_tail_s": time.perf_counter() - t_reads_done,
                        "cold_path": "listing with stat, reads into one exact buffer" + (", each directory uploaded under the next read" if staged else "")}
         return raw, raw_off[:-1].copy(), (raw_off[1:] - raw_off[:-1]), np.zeros(n, dtype=np.int32), staged
@@ -844,38 +858,15 @@ class PackedMemdir:
         raise IndexError(j)
 
     def _raw_arrays(self, segs, order, keep, raw, begin, ln) -> Dict[str, Any]:
-        cols: Dict[str, List[np.ndarray]] = {k: [] for k in ("ts", "wall", "flags8", "spans", "fsb")}
-        names, lens = [], []
-        for key in order:
-            L = segs[key].listing
-            if not L.n:
-                continue
-            cols["ts"].append(L.ts); cols["wall"].append(L.wall); cols["flags8"].append(L.flags8); cols["spans"].append(L.spans)
-            cols["fsb"].append(np.full(L.n, self._fsb_of(key), dtype=np.uint32))
-            names.append(L.names); lens.append((L.name_off[1:] - L.name_off[:-1]).astype(np.int64))
-        n_all = len(keep)
-        cat = lambda k, dt: (np.concatenate(cols[k]) if cols[k] else np.zeros(0, dtype=dt))
-        ts, wall, f8, fsb = cat("ts", np.int64), cat("wall", np.int64), cat("flags8", np.uint64), cat("fsb", np.uint32)
-        spans = np.concatenate(cols["spans"]) if cols["spans"] else np.zeros((0, 4), dtype=np.uint16)
-        nlen = np.concatenate(lens) if lens else np.zeros(0, dtype=np.int64)
-        nblob = b"".join(names)
-        if keep.all():
-            sel_begin, sel_len = begin, ln
-            name = np.frombuffer(nblob, dtype=np.uint8).copy() if nblob else np.zeros(1, dtype=np.uint8)
-            name_off = np.zeros(n_all + 1, dtype=np.uint64); np.cumsum(nlen, out=name_off[1:])
-        else:
+        Ls = [segs[key].listing for key in order]
+        names, name_off = b"".join(L.names for L in Ls), _offsets(_cat([np.diff(L.name_off) for L in Ls], np.uint64))
+        spans, cols = _cat([L.spans for L in Ls], np.uint16, 4), self._columns(segs, order)
+        if not keep.all():
             idx = np.nonzero(keep)[0]
-            noff = np.zeros(n_all + 1, dtype=np.int64); np.cumsum(nlen, out=noff[1:])
-            sel_begin, sel_len = begin[idx], ln[idx]
-            nm = b"".join(nblob[int(noff[j]):int(noff[j + 1])] for j in idx.tolist())
-            name = np.frombuffer(nm, dtype=np.uint8).copy() if nm else np.zeros(1, dtype=np.uint8)
-            name_off = np.zeros(len(idx) + 1, dtype=np.uint64); np.cumsum(nlen[idx], out=name_off[1:])
-            ts, wall, f8, fsb, spans = ts[idx], wall[idx], f8[idx], fsb[idx], spans[idx]
-        n = len(ts)
-        return {"n": n, "global_base": 0, "raw": raw, "raw_bytes": len(raw) if raw is not None else int(self._cold_total), "raw_begin": np.ascontiguousarray(sel_begin, dtype=np.uint64),
-                "raw_len": np.ascontiguousarray(sel_len, dtype=np.uint64), "name": name if n else None,
-                "name_off": name_off if n else None, "name_spans": np.ascontiguousarray(spans.reshape(-1)) if n else None,
-                "ts": np.ascontiguousarray(ts), "wall": np.ascontiguousarray(wall), "flags8": np.ascontiguousarray(f8), "fsb": np.ascontiguousarray(fsb)}
+            names, name_off = _take_names(names, name_off, idx)
+            spans, begin, ln, cols = spans[idx], begin[idx], ln[idx], {k: v[idx] for k, v in cols.items()}
+        return _load_arrays(names, name_off, spans, cols, raw=raw, raw_bytes=len(raw) if raw is not None else int(self._cold_total),
+                            raw_begin=np.ascontiguousarray(begin, dtype=np.uint64), raw_len=np.ascontiguousarray(ln, dtype=np.uint64))
 
     # ---- incremental
     def _incremental(self, changed: List[Tuple[str, str]]) -> None:
@@ -885,16 +876,9 @@ class PackedMemdir:
         rem_key: List[Tuple[int, int, int]] = []
         new_entries: List[Tuple[Tuple[str, str], np.ndarray]] = []
         any_change = False
-        if len(changed) > 1:
-            from concurrent.futures import ThreadPoolExecutor
-            with ThreadPoolExecutor(min(LIST_CONCURRENCY, len(changed))) as ex:
-                listed = list(ex.map(lambda k: self._list(*k), changed))
-        else:
-            listed = [self._list(*k) for k in changed]
-        for key, (listing, mt) in zip(changed, listed):
+        for key, (listing, mt) in zip(changed, self._list_many(changed)):
             old = self.segs.get(key)
-            seg = _Seg(); seg.listing = listing; seg.mtime_ns = mt; seg.bad = list(listing.bad); seg.bad_files = {}; seg.dev = np.full(listing.n, -1, dtype=np.int64)
-            fresh[key] = seg
+            seg = fresh[key] = _new_seg(listing, mt, -1)
             if (old is not None and old.listing.n == listing.n and old.listing.names == listing.names
                     and np.array_equal(old.listing.key(), listing.key())):
                 seg.dev = old.dev                                      # same names, same (inode, size, mtime): nothing to do here
@@ -910,10 +894,10 @@ class PackedMemdir:
                         seg.dev[i] = old.dev[j]; used[j] = True
                 for i in np.nonzero(seg.dev < 0)[0].tolist():          # a file already known to be unpackable, unchanged: stays out, stays reported
                     nb = listing.name_bytes(i)
-                    if old.bad_files.get(nb) == (int(nk_[i]["ino"]), int(nk_[i]["size"]), int(nk_[i]["mtime"])):
+                    if old.bad_files.get(nb) == listing.ident(i):
                         seg.dev[i] = -2; seg.bad_files[nb] = old.bad_files[nb]
                 for j in np.nonzero(~used)[0].tolist():
-                    rem_dev.append(int(old.dev[j])); rem_key.append((int(ok_[j]["ino"]), int(ok_[j]["size"]), int(ok_[j]["mtime"])))
+                    rem_dev.append(int(old.dev[j])); rem_key.append(old.listing.ident(j))
                 if old.bad:                                            # undecodable files that did not change stay reported without being read again
                     seg.bad.extend(m for m in old.bad if m not in seg.bad and self._bad_still_there(key, m, listing))
                 if not used.all() or (seg.dev == -1).any() or not np.array_equal(old.dev, seg.dev[seg.dev != -2]):
@@ -946,10 +930,9 @@ class PackedMemdir:
         to_read: List[Tuple[Tuple[str, str], np.ndarray]] = []
         for key, todo in new_entries:
             L = fresh[key].listing
-            nk_ = L.key()
             still = []
             for i in todo.tolist():
-                d = rem_map.pop((int(nk_[i]["ino"]), int(nk_[i]["size"]), int(nk_[i]["mtime"])), None)
+                d = rem_map.pop(L.ident(i), None)
                 if d is not None:
                     moved_from.append(d); moved_to.append((key, i))
                 else:
@@ -992,8 +975,7 @@ class PackedMemdir:
                 seg.dev[i] = self.n_base + len(kept)
                 kept.append(j)
             else:
-                seg.bad.append(f"Error processing {seg.listing.name(i)}: {_decode_error(raws[j])}")
-                seg.bad_files[seg.listing.name_bytes(i)] = (int(seg.listing.ino[i]), int(seg.listing.size[i]), int(seg.listing.mtime_ns[i]))
+                _report_unpackable(seg, i, raws[j])
                 seg.dev[i] = -2
         for key in self._order():                                      # entries that could not be packed leave the listing
             seg = fresh.get(key) or self.segs.get(key)
@@ -1040,16 +1022,11 @@ class PackedMemdir:
         delta = None
         while any(keep):
             idx = [j for j, k in enumerate(keep) if k]
-            off = np.zeros(len(idx) + 1, dtype=np.uint64)
-            np.cumsum([len(raws[j]) for j in idx], out=off[1:])
+            off = _offsets([len(raws[j]) for j in idx])
             raw = np.frombuffer(b"".join(raws[j] for j in idx), dtype=np.uint8).copy() if off[-1] else np.zeros(1, dtype=np.uint8)
-            names = [metas[j][0] for j in idx]
-            name_off = np.zeros(len(idx) + 1, dtype=np.uint64); np.cumsum([len(x) for x in names], out=name_off[1:])
-            arrays = {"n": len(idx), "global_base": 0, "raw": raw, "raw_off": off,
-                      "name": np.frombuffer(b"".join(names), dtype=np.uint8).copy(), "name_off": name_off,
-                      "name_spans": np.array([metas[j][4] for j in idx], dtype=np.uint16).reshape(-1),
-                      "ts": np.array([metas[j][1] for j in idx], dtype=np.int64), "wall": np.array([metas[j][2] for j in idx], dtype=np.int64),
-                      "flags8": np.array([metas[j][3] for j in idx], dtype=np.uint64), "fsb": np.array([metas[j][5] for j in idx], dtype=np.uint32)}
+            names, ts, wall, f8, spans, fsb = zip(*(metas[j] for j in idx))
+            arrays = _load_arrays(b"".join(names), _offsets([len(x) for x in names]), spans, {"ts": ts, "wall": wall, "flags8": f8, "fsb": fsb},
+                                  raw=raw, raw_off=off)
             if delta is None:
                 delta = Corpus()
             valid = delta.load_raw(arrays)
@@ -1063,27 +1040,27 @@ class PackedMemdir:
         return None, keep
 
     # ---- listing order
+    def _columns(self, segs, keys) -> Dict[str, np.ndarray]:
+        """The meta columns of these directories' entries, in listing order (fsb without the record bits)."""
+        Ls = [segs[key].listing for key in keys]
+        cols = {k: _cat([getattr(L, k) for L in Ls], _META_COLS[k]) for k in ("ts", "wall", "flags8")}
+        cols["fsb"] = _cat([np.full(L.n, self._fsb_of(key), dtype=np.uint32) for key, L in zip(keys, Ls)], np.uint32)
+        return cols
+
     def _rebuild_listing(self) -> None:
+        order = self._order()
         self.segments = {}
         pos = 0
-        devs: List[np.ndarray] = []
-        cols: Dict[str, List[np.ndarray]] = {k: [] for k in ("ts", "wall", "flags8", "fsb")}
-        for key in self._order():
-            seg = self.segs[key]
-            k = seg.listing.n
+        for key in order:
+            k = self.segs[key].listing.n
             self.segments[key] = (pos, pos + k)
             pos += k
-            if k:
-                devs.append(seg.dev)
-                cols["ts"].append(seg.listing.ts); cols["wall"].append(seg.listing.wall); cols["flags8"].append(seg.listing.flags8)
-                cols["fsb"].append(np.full(k, self._fsb_of(key), dtype=np.uint32))
         self.n = pos
-        self.dev = np.concatenate(devs) if devs else np.zeros(0, dtype=np.int64)
+        self.dev = _cat([self.segs[key].dev for key in order], np.int64)
         self.pos_of_dev = np.full(self.n_base + self.n_delta, -1, dtype=np.int64)
         self.pos_of_dev[self.dev] = np.arange(self.n, dtype=np.int64)
         self.identity = self.n == self.n_base and self.n_delta == 0 and bool((self.dev == np.arange(self.n)).all())
-        dts = {"ts": np.int64, "wall": np.int64, "flags8": np.uint64, "fsb": np.uint32}
-        self.arrays = {k: (np.concatenate(v) if v else np.zeros(0, dtype=dts[k])) for k, v in cols.items()}
+        self.arrays = self._columns(self.segs, order)
         bits = np.zeros(self.n_base + self.n_delta, dtype=np.uint8)
         for corpus, lo in self._corpora():
             if corpus.n:
@@ -1115,7 +1092,7 @@ class PackedMemdir:
                 per[q].append(h.astype(np.int64) + lo)
         out = []
         for q in range(nq):
-            ids = np.concatenate(per[q]) if per[q] else np.zeros(0, dtype=np.int64)
+            ids = _cat(per[q], np.int64)
             if not self.identity:
                 ids = self.pos_of_dev[ids]
                 ids = ids[ids >= 0]
@@ -1329,7 +1306,8 @@ class PackedMemdir:
             for a in ("name_off", "ts", "wall", "flags8", "spans", "ino", "size", "mtime_ns"):
                 setattr(L, a, z[f"s{k}_{a}"])
             L.n = len(L.ts); L.bad = []
-            seg = _Seg(); seg.listing = L; seg.dev = np.arange(pos, pos + L.n, dtype=np.int64); seg.mtime_ns = -2; seg.bad = [str(x) for x in z[f"s{k}_bad"]]; seg.bad_files = {}
+            seg = _new_seg(L, -2, 0)
+            seg.dev = np.arange(pos, pos + L.n, dtype=np.int64); seg.bad = [str(x) for x in z[f"s{k}_bad"]]
             pos += L.n
             pm.segs[key] = seg
         pm.corpus = Corpus()
@@ -1349,9 +1327,7 @@ class PackedMemdir:
 
 def _subset(L: DirListing, sel: np.ndarray) -> DirListing:
     d = DirListing()
-    d.names = b"".join(L.name_bytes(i) for i in sel.tolist())
-    d.name_off = np.zeros(len(sel) + 1, dtype=np.uint64)
-    np.cumsum((L.name_off[1:] - L.name_off[:-1])[sel], out=d.name_off[1:])
+    d.names, d.name_off = _take_names(L.names, L.name_off, sel)
     for k in ("ts", "wall", "flags8", "spans", "ino", "size", "mtime_ns"):
         setattr(d, k, getattr(L, k)[sel])
     d.n = len(sel)
@@ -1407,9 +1383,7 @@ def arrays_from_segments(recs: Sequence[Dict[str, Any]], folder_ids: Dict[str, i
     name_parts = [os.fsencode(r["filename"]) for r in recs]
 
     def blob(parts):
-        off = np.zeros(n + 1, dtype=np.uint64)
-        if n:
-            np.cumsum(np.fromiter(map(len, parts), dtype=np.int64, count=n), out=off[1:])
+        off = _offsets(np.fromiter(map(len, parts), dtype=np.int64, count=n))
         data = np.frombuffer(b"".join(parts), dtype=np.uint8).copy() if n and off[n] else np.zeros(1, dtype=np.uint8)
         return data, off
 
