@@ -9,14 +9,15 @@ import io
 import os
 import re
 import struct
+from datetime import datetime, timezone
 
 import numpy as np
 import pytest
 
 from fei_b200 import program as P
 from fei_b200 import synth
-from fei_b200.program import (C_BODY, C_FLAGS, C_FOLDER_SET, C_NAME, C_SLOT, NAME_FILENAME, NAME_ID, NAME_TS_STR, VERSION_NFA, Cond,
-                              ProgramBuilder)
+from fei_b200.program import (C_BODY, C_FLAGS, C_FOLDER_SET, C_NAME, C_SLOT, NAME_DATE_STR, NAME_FILENAME, NAME_HOST, NAME_ID, NAME_TS_STR,
+                              VERSION_NFA, Cond, ProgramBuilder)
 from fei_b200.regexc import Pattern
 from tests.blob_nfa_model import BlobNfa
 
@@ -99,6 +100,10 @@ def _value(rec, head, c):
     if c.kind == C_FLAGS:
         return rec["flags"]
     if c.kind == C_NAME:
+        if c.which == NAME_HOST:                                         # "ts.uid.host:2,flags"
+            return rec["filename"].split(".", 2)[2].rsplit(":2,", 1)[0]
+        if c.which == NAME_DATE_STR:                                     # str(datetime.fromtimestamp(ts)) of the wall clock
+            return str(datetime.fromtimestamp(rec.get("wall", rec["ts"]), timezone.utc).replace(tzinfo=None))
         return {NAME_FILENAME: rec["filename"], NAME_ID: rec["uid"], NAME_TS_STR: str(rec["ts"])}[c.which]
     return rec["body"].decode()
 
