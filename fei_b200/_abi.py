@@ -58,7 +58,7 @@ class ScanTiming(C.Structure):
                 ("d2h_ms", C.c_float), ("total_ms", C.c_float), ("kernel_launches", C.c_uint32),
                 ("body_bytes_touched", C.c_uint64), ("body_bytes_read", C.c_uint64),
                 ("body_kernel", C.c_uint32), ("body_direct", C.c_uint32), ("body_acc_mode", C.c_uint32),
-                ("body_nfa_words", C.c_uint32)]
+                ("body_nfa_words", C.c_uint32), ("body_nfa_counters", C.c_uint32)]
 
 
 class DirlistView(C.Structure):

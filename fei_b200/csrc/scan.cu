@@ -156,16 +156,60 @@ struct NfaTables {
   }
 };
 
-template <int W>
+// Counter positions of a content automaton (feiscan_prog.h fei_prog_nfa_ctr), all in registers: position, bound and age of
+// each.  Empty for the automata without counters.
+template <bool kCtr> struct NfaCounters {};
+template <> struct NfaCounters<true> {
+  uint32_t n, pos[FEI_NFA_MAX_COUNTERS], bound[FEI_NFA_MAX_COUNTERS], age[FEI_NFA_MAX_COUNTERS];
+};
+
+template <int W, bool kCtr = false>
 struct Nfa {
   uint32_t d[W];                     // active positions
   uint32_t prev;                     // context kind of the last code point (0: none yet)
   uint32_t cp, need;                 // UTF-8 decoder: code point so far, continuation bytes still to come
   uint32_t acc;                      // output bits of the accepts met so far (end-only accepts not included)
+  NfaCounters<kCtr> ctr;
+  // kCtr: the counter table (uint32[n][2]: position, bound), read once into registers
+  __device__ __forceinline__ void load_counters(const uint32_t* tab, uint32_t n) {
+    ctr.n = n;
+#pragma unroll
+    for (int i = 0; i < FEI_NFA_MAX_COUNTERS; ++i) {
+      ctr.pos[i] = i < (int)n ? tab[2 * i] : 0u;
+      ctr.bound[i] = i < (int)n ? tab[2 * i + 1] : 0u;
+    }
+  }
   __device__ __forceinline__ void reset(const NfaTables& t) {
 #pragma unroll
     for (int k = 0; k < W; ++k) d[k] = t.masks[2 * W + k];
     prev = 0; cp = 0; need = 0; acc = 0;
+    if constexpr (kCtr) {
+#pragma unroll
+      for (int i = 0; i < FEI_NFA_MAX_COUNTERS; ++i) ctr.age[i] = 0;
+    }
+  }
+  // kCtr: n = Follow(D, ctx) gets the counter positions that continue their run, D[P] && age_P < k, and every age steps
+  // (1 on entry).  A position's word is a run-time value: d[] and n[] are read and written with unrolled compares, so they
+  // stay in registers.
+  __device__ __forceinline__ void count(uint32_t* n) {
+    uint32_t keep[W];
+#pragma unroll
+    for (int k = 0; k < W; ++k) keep[k] = 0;
+#pragma unroll
+    for (int i = 0; i < FEI_NFA_MAX_COUNTERS; ++i) {
+      if (i < (int)ctr.n) {
+        const uint32_t w = ctr.pos[i] >> 5, m = 1u << (ctr.pos[i] & 31u);
+        uint32_t fw = 0, dw = 0;
+#pragma unroll
+        for (int k = 0; k < W; ++k) if (k == (int)w) { fw = n[k]; dw = d[k]; }
+        const uint32_t cont = (dw & m) && ctr.age[i] < ctr.bound[i] ? m : 0u;
+        ctr.age[i] = (fw & m) ? 1u : ctr.age[i] + 1u;
+#pragma unroll
+        for (int k = 0; k < W; ++k) if (k == (int)w) keep[k] |= cont;
+      }
+    }
+#pragma unroll
+    for (int k = 0; k < W; ++k) n[k] |= keep[k];
   }
   __device__ __forceinline__ bool any(const uint32_t* src) const {
     uint32_t x = 0;
@@ -200,6 +244,7 @@ struct Nfa {
         for (int k = 0; k < W; ++k) n[k] |= r[W + k];
       }
     }
+    if constexpr (kCtr) count(n);
     const uint32_t* b = t.cls_b + (ck & 0xFFu) * W;
 #pragma unroll
     for (int k = 0; k < W; ++k) d[k] = n[k] & b[k];
@@ -1574,8 +1619,10 @@ __global__ void __launch_bounds__(kBodyThreads, 1) k_body_gather(BodyArgs a, con
 // skipped); each lane undoes the tile byte permutation, decodes UTF-8 and looks the class up (ASCII table, else a binary
 // search over the range table).  A program that also has a body DFA (class-indexed, not sticky) steps it on every byte as
 // k_body<false, 0> does; its outputs are the content bits below the automaton's first_bit.  The ordered lists are compacted
-// after the scan and the multi-GPU hook copies the masks (no window work in the kernel).
-template <int W> struct NfaThreads { static constexpr int value = W <= 4 ? 1024 : 512; };
+// after the scan and the multi-GPU hook copies the masks (no window work in the kernel).  kCtr: the automaton has counter
+// positions (version-3 programs, feiscan_prog.h fei_prog_nfa_ctr); their positions, bounds and ages take 25 more registers, so
+// those instances run 512 threads per CTA (128 registers) at every W.
+template <int W, bool kCtr = false> struct NfaThreads { static constexpr int value = W <= 4 && !kCtr ? 1024 : 512; };
 
 // Stage the body DFA's tables (bytes0, may be 0) and the position automaton's behind them with one mbarrier.
 __device__ __forceinline__ void stage_two_tables(uint8_t* dst0, const uint8_t* src0, uint32_t bytes0, uint8_t* dst1, const uint8_t* src1,
@@ -1590,8 +1637,8 @@ __device__ __forceinline__ void stage_two_tables(uint8_t* dst0, const uint8_t* s
   mbar_wait(bar, 0);
 }
 
-template <int W, bool kHasDfa>
-__global__ void __launch_bounds__(NfaThreads<W>::value, 1) k_body_nfa(BodyArgs a) {
+template <int W, bool kHasDfa, bool kCtr>
+__global__ void __launch_bounds__(NfaThreads<W, kCtr>::value, 1) k_body_nfa(BodyArgs a) {
   extern __shared__ __align__(128) uint8_t smem[];
   __shared__ uint64_t bar;
   __shared__ uint32_t q_need[33];                  // as in k_body
@@ -1625,7 +1672,11 @@ __global__ void __launch_bounds__(NfaThreads<W>::value, 1) k_body_nfa(BodyArgs a
     endout = reinterpret_cast<const uint32_t*>(smem + (dd->off_endout - dd->off_trans));
     dfa_start = dd->start;
   }
-  Nfa<W> nfa;
+  Nfa<W, kCtr> nfa;
+  if constexpr (kCtr) {                            // check_prog: the descriptor right behind the section, its table staged with it
+    const fei_prog_nfa_ctr* cd = reinterpret_cast<const fei_prog_nfa_ctr*>(a.prog + ph->off_body_nfa + sizeof(fei_prog_nfa));
+    nfa.load_counters(reinterpret_cast<const uint32_t*>(nsm + (cd->off_counters - nd->off_ascii)), cd->n_counters);
+  }
   const uint32_t all_q = nq >= 32 ? 0xFFFFFFFFu : ((1u << nq) - 1u);
   const int lane = threadIdx.x & 31;
   unsigned long long touched = 0;
@@ -1698,15 +1749,21 @@ __global__ void __launch_bounds__(NfaThreads<W>::value, 1) k_body_nfa(BodyArgs a
 }
 
 using BodyKernel = void (*)(BodyArgs);
-static BodyKernel body_nfa_kernel(uint32_t words, bool has_dfa) {
+template <bool kCtr> static BodyKernel body_nfa_kernel(uint32_t words, bool has_dfa) {
   switch (words) {
-    case 1: return has_dfa ? k_body_nfa<1, true> : k_body_nfa<1, false>;
-    case 2: return has_dfa ? k_body_nfa<2, true> : k_body_nfa<2, false>;
-    case 4: return has_dfa ? k_body_nfa<4, true> : k_body_nfa<4, false>;
-    default: return has_dfa ? k_body_nfa<8, true> : k_body_nfa<8, false>;
+    case 1: return has_dfa ? k_body_nfa<1, true, kCtr> : k_body_nfa<1, false, kCtr>;
+    case 2: return has_dfa ? k_body_nfa<2, true, kCtr> : k_body_nfa<2, false, kCtr>;
+    case 4: return has_dfa ? k_body_nfa<4, true, kCtr> : k_body_nfa<4, false, kCtr>;
+    default: return has_dfa ? k_body_nfa<8, true, kCtr> : k_body_nfa<8, false, kCtr>;
   }
 }
-static int body_nfa_threads(uint32_t words) { return words == 8 ? NfaThreads<8>::value : NfaThreads<4>::value; }
+static BodyKernel body_nfa_kernel(uint32_t words, bool has_dfa, bool counters) {
+  return counters ? body_nfa_kernel<true>(words, has_dfa) : body_nfa_kernel<false>(words, has_dfa);
+}
+static int body_nfa_threads(uint32_t words, bool counters) {
+  if (counters) return words == 8 ? NfaThreads<8, true>::value : NfaThreads<4, true>::value;
+  return words == 8 ? NfaThreads<8>::value : NfaThreads<4>::value;
+}
 
 // The content kernel of one scan: k_body_sticky when the sticky automaton's row addresses fit 16 bits, else the k_body
 // instance for the table's column mapping and accumulator mode.
@@ -1855,7 +1912,7 @@ __global__ void __launch_bounds__(256) k_list_checksum(const T* __restrict__ v, 
 static int check_prog(const uint8_t* prog, uint64_t len) {
   if (!prog || len < sizeof(fei_prog_hdr)) { set_error("program blob too small"); return FEI_E_BADARG; }
   fei_prog_hdr h; memcpy(&h, prog, sizeof(h));
-  if (h.magic != FEI_PROG_MAGIC || (h.version != FEI_PROG_VERSION && h.version != FEI_PROG_VERSION_NFA)) { set_error("bad program magic/version"); return FEI_E_BADARG; }
+  if (h.magic != FEI_PROG_MAGIC || (h.version != FEI_PROG_VERSION && h.version != FEI_PROG_VERSION_NFA && h.version != FEI_PROG_VERSION_CTR)) { set_error("bad program magic/version"); return FEI_E_BADARG; }
   if (h.total_bytes != len) { set_error("program length mismatch (%u vs %llu)", h.total_bytes, (unsigned long long)len); return FEI_E_BADARG; }
   if (h.n_queries == 0 || h.n_queries > FEI_MAX_QUERIES) { set_error("1..32 queries per program"); return FEI_E_BADARG; }
   if (h.n_slots > FEI_MAX_SLOTS) { set_error("at most %d header slots per program", FEI_MAX_SLOTS); return FEI_E_UNSUPPORTED; }
@@ -1917,7 +1974,26 @@ static int check_prog(const uint8_t* prog, uint64_t len) {
     if (!ok) { set_error("bad flags / name position automaton in program"); return FEI_E_BADARG; }
   }
   if (!nfa_ok(h.off_body_nfa, false)) { set_error("bad content position automaton in program"); return FEI_E_BADARG; }
-  if ((h.version == FEI_PROG_VERSION_NFA) != (n_nfa != 0)) { set_error("bad program magic/version"); return FEI_E_BADARG; }
+  if ((h.version != FEI_PROG_VERSION) != (n_nfa != 0)) { set_error("bad program magic/version"); return FEI_E_BADARG; }
+  // counters: version 3 if and only if the content automaton has a fei_prog_nfa_ctr (the head ones never have one)
+  if (h.version == FEI_PROG_VERSION_CTR) {
+    fei_prog_nfa a; fei_prog_nfa_ctr cd;
+    const uint64_t at = (uint64_t)h.off_body_nfa + sizeof(a);
+    bool ok = h.off_body_nfa != 0 && in(at, sizeof(cd));
+    if (ok) {
+      memcpy(&a, prog + h.off_body_nfa, sizeof(a)); memcpy(&cd, prog + at, sizeof(cd));
+      const uint64_t W = a.n_words, end = (uint64_t)a.off_ascii + a.table_bytes;
+      ok = a.off_ascii >= at + sizeof(cd) && cd.n_counters >= 1 && cd.n_counters <= FEI_NFA_MAX_COUNTERS &&
+           cd.off_counters % 16 == 0 && cd.off_counters >= a.off_ascii && cd.off_counters + 8ull * cd.n_counters <= end;
+      const uint32_t* tab = reinterpret_cast<const uint32_t*>(prog + cd.off_counters);
+      const uint32_t* self_loop = reinterpret_cast<const uint32_t*>(prog + a.off_masks) + W;
+      for (uint32_t i = 0; i < cd.n_counters && ok; ++i) {
+        const uint32_t pos = tab[2 * i], bound = tab[2 * i + 1];
+        ok = pos >= 1 && pos < a.n_pos && !(self_loop[pos >> 5] >> (pos & 31u) & 1u) && bound >= 1;
+      }
+    }
+    if (!ok) { set_error("bad counters of the content position automaton in program"); return FEI_E_BADARG; }
+  }
   if (h.off_body_nfa) {
     fei_prog_dfa d{};
     if (h.off_body_dfa) memcpy(&d, prog + h.off_body_dfa, sizeof(d));
@@ -2063,6 +2139,8 @@ int run_scan(fei_corpus* c, const uint8_t* prog, uint64_t prog_len, int compact_
     if (smem > 220 * 1024) { set_error("content automata need %zu bytes of shared memory (limit 220 KiB)", smem); return FEI_E_UNSUPPORTED; }
     c->timing.body_kernel = 4u;
     c->timing.body_nfa_words = na.n_words;
+    if (h.version == FEI_PROG_VERSION_CTR)
+      c->timing.body_nfa_counters = reinterpret_cast<const fei_prog_nfa_ctr*>(prog + h.off_body_nfa + sizeof(fei_prog_nfa))->n_counters;
   } else if (n && need_body) {
     memcpy(&d, prog + h.off_body_dfa, sizeof(d));
     smem = d.table_bytes;
@@ -2114,7 +2192,8 @@ int run_scan(fei_corpus* c, const uint8_t* prog, uint64_t prog_len, int compact_
   }
   if (push) { a.push_peers = hook->push_peers; a.push_n = hook->push_n; a.push_off = hook->push_off; hook->pushed = true; }
   if (n && nfa) {
-    FEI_TRY(launch_body_nfa(body_nfa_kernel(na.n_words, h.off_body_dfa != 0), body_nfa_threads(na.n_words), grid, smem, s, a));
+    const bool counters = c->timing.body_nfa_counters != 0;
+    FEI_TRY(launch_body_nfa(body_nfa_kernel(na.n_words, h.off_body_dfa != 0, counters), body_nfa_threads(na.n_words, counters), grid, smem, s, a));
     ++launches;
   } else if (n && need_body) {
     const size_t body_smem = sticky_kernel ? ((smem + 127) & ~(size_t)127) + kStickyRingBytes : smem;   // k_body_sticky: + its rings

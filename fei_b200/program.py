@@ -12,9 +12,9 @@ from typing import Dict, List, Optional, Sequence, Tuple
 
 import numpy as np
 
-from .regexc import Dfa, Pattern, PatternTooLarge, Pna, compile_patterns, compile_positions
+from .regexc import Dfa, Pattern, PatternTooLarge, Pna, compile_patterns, compile_positions, compile_positions_counted
 
-MAGIC, VERSION, VERSION_NFA = 0x50494546, 1, 2
+MAGIC, VERSION, VERSION_NFA, VERSION_CTR = 0x50494546, 1, 2, 3
 C_CONST, C_BODY, C_SLOT, C_FLAGS, C_NAME, C_DATE_CMP, C_FOLDER_SET, C_STATUS_SET, C_RECBITS, C_TS_CMP = range(10)
 CMP = {">": 0, "<": 1, ">=": 2, "<=": 3, "=": 4, "!=": 5}
 NAME_FILENAME, NAME_ID, NAME_HOST, NAME_TS_STR, NAME_DATE_STR = 0, 1, 2, 3, 4     # 3 / 4: str(metadata["timestamp"]) / str(metadata["date"]), formatted by the kernels
@@ -57,6 +57,7 @@ def _pad16(b: bytearray) -> None:
 _DFA_CACHE: Dict[Tuple, Dfa] = {}
 _DFA_FAIL: Dict[Tuple, str] = {}       # same keys: pattern sets whose DFA was refused (PatternTooLarge), with the reason
 _PNA_CACHE: Dict[Tuple, Pna] = {}
+_PNA_CTR_CACHE: Dict[Tuple, Pna] = {}
 
 
 def _remember(cache: Dict, key, value) -> None:
@@ -98,6 +99,25 @@ def cached_positions(patterns: Sequence[Pattern]) -> Pna:
     return a
 
 
+def cached_counted_positions(patterns: Sequence[Pattern]) -> Pna:
+    """compile_positions_counted, cached per process like cached_positions."""
+    key = tuple(_pkey(p) for p in patterns)
+    a = _PNA_CTR_CACHE.get(key)
+    if a is None:
+        a = compile_positions_counted(patterns)
+        _remember(_PNA_CTR_CACHE, key, a)
+    return a
+
+
+def content_positions(patterns: Sequence[Pattern]) -> Pna:
+    """The position automaton of content patterns: the plain one, or the one with counters where the plain one is refused
+    (long bounded gaps such as `a.{0,1000}b`)."""
+    try:
+        return cached_positions(patterns)
+    except PatternTooLarge:
+        return cached_counted_positions(patterns)
+
+
 def content_automaton(p: Pattern):
     """The automaton one pattern runs on the host: its DFA, or its position automaton when the DFA is refused.  Both have
     .run(bytes) -> mask: the empty-string verdict of a content condition without with_content, and the folder / status names
@@ -105,7 +125,7 @@ def content_automaton(p: Pattern):
     try:
         return cached_dfa([p])
     except PatternTooLarge:
-        return cached_positions([p])
+        return content_positions([p])
 
 
 class _FieldDfa:
@@ -206,7 +226,7 @@ def _table_bytes(d: Dfa, direct_limit: int) -> int:
 
 def serialize_nfa(a: Pna, blob: bytearray, first_bit: int) -> int:
     """Append a fei_prog_nfa section (include/feiscan_prog.h); returns its offset.  Output bit k of the automaton becomes
-    content bit first_bit + k."""
+    content bit first_bit + k.  An automaton with counters (content only) gets a fei_prog_nfa_ctr right behind the descriptor."""
     W = a.n_words
     if first_bit + a.n_patterns > 32:
         raise NotImplementedError("more than 32 content patterns in one program")
@@ -221,7 +241,7 @@ def serialize_nfa(a: Pna, blob: bytearray, first_bit: int) -> int:
 
     _pad16(blob)
     desc_off = len(blob)
-    blob.extend(b"\0" * 64)
+    blob.extend(b"\0" * (80 if a.counters else 64))                               # + fei_prog_nfa_ctr
     ck = lambda c: c | a.cls_kind[c] << 8                                          # noqa: E731
     off_ascii = table(np.array([ck(c) for c in a.ascii_cls], dtype=np.uint16))
     off_lo = table(np.array([lo for lo, _c in a.ranges], dtype=np.uint32))
@@ -231,6 +251,9 @@ def serialize_nfa(a: Pna, blob: bytearray, first_bit: int) -> int:
     off_follow = table(np.array([w for src, dst, m in a.follow for w in words(src) + words(dst) + [m]], dtype=np.uint32))
     off_accept = table(np.array([w for src, m, p, eo in a.accept for w in words(src) + [m, (first_bit + p) | (int(eo) << 8)]],
                                 dtype=np.uint32))
+    if a.counters:                   # the counter table is the last of the contiguous tables
+        off_ctr = table(np.array([x for pk in a.counters for x in pk], dtype=np.uint32))
+        struct.pack_into("<4I", blob, desc_off + 64, len(a.counters), off_ctr, 0, 0)
     struct.pack_into("<16I", blob, desc_off, W, a.n_pos, len(a.cls_b), len(a.ranges), len(a.follow), len(a.accept), a.n_patterns,
                      first_bit, off_ascii, off_lo, off_rck, off_b, off_masks, off_follow, off_accept, len(blob) - off_ascii)
     return desc_off
@@ -242,7 +265,9 @@ def _route(patterns: Sequence[Pattern], fits, sticky: bool = False) -> Tuple[Lis
     automaton.  Otherwise every pattern whose DFA is refused (or does not fit) on its own goes to the position automaton, and
     then the patterns with the largest DFAs until the union of the rest fits.  The field's size rule is
     fits(dfa, pna, whole): whether `dfa` fits next to position automaton `pna` (None: alone); `whole` marks the first try,
-    the union compiled with `sticky`."""
+    the union compiled with `sticky`.  Content (fits is _body_fits) takes the automaton with counters where the plain one is
+    refused; head fields keep the plain one."""
+    positions = content_positions if fits is _body_fits else cached_positions
     idx = list(range(len(patterns)))
     try:
         if fits(cached_dfa(patterns, sticky=sticky), None, True):
@@ -260,7 +285,7 @@ def _route(patterns: Sequence[Pattern], fits, sticky: bool = False) -> Tuple[Lis
     dfa = [i for i in idx if i in size]
     while True:
         nfa = [i for i in idx if i not in dfa]
-        a = cached_positions([patterns[i] for i in nfa])
+        a = positions([patterns[i] for i in nfa])
         if not dfa:
             break
         try:
@@ -420,7 +445,7 @@ class ProgramBuilder:
         if tb > BODY_SMEM_LIMIT:
             raise NotImplementedError(f"content automaton needs {tb} bytes of shared memory (limit 220 KiB)")
         _pad16(blob)
-        version = VERSION_NFA if any(nfa for _dfa, nfa, _a in routes.values()) else VERSION
+        version = VERSION_CTR if pna is not None and pna.counters else VERSION_NFA if any(nfa for _dfa, nfa, _a in routes.values()) else VERSION
         struct.pack_into("<22I", blob, 0, MAGIC, version, len(blob), len(self.queries), len(recs), off_conds,
                          off_queries, len(slots), off_slots, off_key, off_body, off_flags, off_names[0], off_names[1], off_names[2],
                          head_mask, body_mask, slot_mask, name_mask, head_bytes, off_names[3], off_names[4])

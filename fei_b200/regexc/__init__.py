@@ -158,6 +158,7 @@ class Nfa:
         self.uses: set = set()
         self.dollar_edges: List[Tuple[int, int]] = []   # non-multiline `$` edges (need the trailing-newline rule)
         self.end_only: set = set()                      # states whose accept only counts at end of input
+        self.bound: Dict[Tuple[int, int, int], int] = {}   # counter edges (src, leaf, dst) -> k: `leaf{1,k}` as one edge
 
     def new(self) -> int:
         self.eps.append([]); self.chars.append([])
@@ -214,11 +215,52 @@ class Nfa:
         self.uses.add(A_NEXTNL)
 
 
-class _RegexBuilder:
-    """re._parser AST -> NFA fragment (Thompson construction)."""
+def _single_leaf(p, flags: int):
+    """(leaf node, its flags) when repeat body `p` is one character leaf, possibly inside groups or inline-flag groups."""
+    while len(p) == 1:
+        op, av = p[0]
+        if op in (_K.LITERAL, _K.NOT_LITERAL, _K.ANY, _K.IN):
+            return p[0], flags
+        if op is not _K.SUBPATTERN:
+            return None
+        _group, add, dele, p = av
+        flags = (flags | add) & ~dele
+    return None
 
-    def __init__(self, nfa: Nfa):
+
+def _countable(node, flags: int) -> bool:
+    """A repeat a counter can hold: `C{lo,hi}` with a finite hi > lo and one character leaf C."""
+    op, av = node
+    if op not in (_K.MAX_REPEAT, _K.MIN_REPEAT):
+        return False
+    lo, hi, p = av
+    return hi is not MAXREPEAT and hi != MAXREPEAT and hi > lo and _single_leaf(p, flags) is not None
+
+
+def _countable_repeats(items, flags: int, out: list) -> list:
+    """Countable repeats of an AST in a fixed depth-first order: [(node, hi - lo)].  Repeats inside a countable one are not
+    visited (its body is a single character)."""
+    for node in items:
+        op, av = node
+        if _countable(node, flags):
+            out.append((node, av[1] - av[0]))
+        elif op is _K.SUBPATTERN:
+            _countable_repeats(av[3], (flags | av[1]) & ~av[2], out)
+        elif op is _K.BRANCH:
+            for alt in av[1]:
+                _countable_repeats(alt, flags, out)
+        elif op in (_K.MAX_REPEAT, _K.MIN_REPEAT):
+            _countable_repeats(av[2], flags, out)
+    return out
+
+
+class _RegexBuilder:
+    """re._parser AST -> NFA fragment (Thompson construction).  `counted`: ids of the countable repeat nodes that become one
+    counter edge each (compile_positions_counted) instead of hi expanded copies."""
+
+    def __init__(self, nfa: Nfa, counted: FrozenSet[int] = frozenset()):
         self.n = nfa
+        self.counted = counted
 
     def seq(self, items, flags: int, a: int) -> int:
         cur = a
@@ -245,6 +287,18 @@ class _RegexBuilder:
         if op in (_K.MAX_REPEAT, _K.MIN_REPEAT):
             lo, hi, p = av
             cur = a
+            if id(node) in self.counted:             # lo copies, then C{0,hi-lo} as the epsilon bypass and one counter edge
+                if lo > 1000:
+                    raise PatternTooLarge("repeat count above 1000")
+                for _ in range(lo):
+                    cur = self.seq(p, flags, cur)
+                leaf, lflags = _single_leaf(p, flags)
+                t = n.new(); out = n.new()
+                rs = regex_leaf_set(leaf, lflags)
+                n.c(cur, rs, t)
+                n.bound[(cur, n.leaf(rs), t)] = hi - lo
+                n.e(cur, out); n.e(t, out)
+                return out
             if lo > 1000 or (hi is not MAXREPEAT and hi > 1000):
                 raise PatternTooLarge("repeat count above 1000")
             for _ in range(lo):
@@ -476,8 +530,9 @@ def _add_sigma_exact(n: Nfa, pid: int, pat: Pattern) -> None:
     n.e(n.start, P(f.start, 0, ""))
 
 
-def add_pattern(n: Nfa, pid: int, pat: Pattern, _plain: bool = False) -> None:
-    """Attach pattern `pid` to the union NFA.  `n.start` is the global start (position 0 only)."""
+def add_pattern(n: Nfa, pid: int, pat: Pattern, _plain: bool = False, counted: Sequence[int] = ()) -> None:
+    """Attach pattern `pid` to the union NFA.  `n.start` is the global start (position 0 only).  counted (regex only): indices
+    into _countable_repeats of the pattern's AST of the repeats built as counter edges."""
     k = pat.kind
     if not _plain and k in ("contains", "startswith", "endswith", "equals", "has_tag") and ("\u03c3" in pat.text or "\u03c2" in pat.text):
         _add_sigma_exact(n, pid, pat)
@@ -491,7 +546,11 @@ def add_pattern(n: Nfa, pid: int, pat: Pattern, _plain: bool = False) -> None:
         n.e(n.start, u)
         n.c(u, _ANY_ALL, u)
         s = n.new(); n.e(u, s)
-        end = _RegexBuilder(n).seq(ast.data, flags, s)
+        ids = frozenset()
+        if counted:
+            reps = _countable_repeats(ast.data, flags, [])
+            ids = frozenset(id(reps[i][0]) for i in counted)
+        end = _RegexBuilder(n, ids).seq(ast.data, flags, s)
         n.accept[end] = pid
         return
     if k in ("contains", "exact_contains"):
@@ -944,6 +1003,7 @@ PNA_MAX_CLASSES = 128
 PNA_MAX_RANGES = 4096        # non-ASCII code point ranges (binary-searched in shared memory)
 PNA_MAX_FOLLOW = 64
 PNA_MAX_ACCEPT = 64
+PNA_MAX_COUNTERS = 8         # counter positions (compile_positions_counted), each with its age in a register of the kernel
 
 
 def ctx_bit(prev_kind: int, next_kind: int) -> int:
@@ -990,6 +1050,7 @@ class Pna:
     start: int
     follow: List[Tuple[int, int, int]]        # (src, dst, ctx mask)
     accept: List[Tuple[int, int, int, bool]]  # (src, ctx mask, pattern, end only)
+    counters: List[Tuple[int, int]] = field(default_factory=list)   # (position, bound k): position P holds `C{1,k}` (see run)
 
     def cls_of(self, cp: int) -> int:
         if cp < 0x80:
@@ -1018,14 +1079,25 @@ class Pna:
         return acc
 
     def run(self, data: bytes) -> int:
-        """Host simulation: mask of matching patterns for `data` (valid UTF-8), like Dfa.run."""
+        """Host simulation: mask of matching patterns for `data` (valid UTF-8), like Dfa.run.  A counter position P with bound k
+        stays set while its class keeps matching and its age (code points since the newest entry) is below k:
+            entered = F[P];  D'[P] = B[P] && (entered || (D[P] && age < k));  age = entered ? 1 : age + 1"""
         d, prev, acc = self.start, K_EDGE, 0
+        age = [0] * len(self.counters)
         for ch in data.decode("utf-8", "surrogatepass"):
             c = self.cls_of(ord(ch))
             kind = self.cls_kind[c]
             ctx = ctx_bit(prev, kind)
             acc |= self.accepts(d, ctx, False)
-            d = self.follow_of(d, ctx) & self.cls_b[c]
+            f = self.follow_of(d, ctx)
+            nd = f
+            for i, (p, k) in enumerate(self.counters):
+                bit = 1 << p
+                entered = f & bit
+                if d & bit and age[i] < k:
+                    nd |= bit
+                age[i] = 1 if entered else age[i] + 1
+            d = nd & self.cls_b[c]
             prev = kind
         return acc | self.accepts(d, ctx_bit(prev, K_EDGE), True)
 
@@ -1062,10 +1134,48 @@ def compile_positions(patterns: Sequence[Pattern]) -> Pna:
     for pid, p in enumerate(patterns):
         add_pattern(n, pid, p)
     n.add_trailing_newline_rule()
+    return _pna_of(n, len(patterns))
+
+
+def compile_positions_counted(patterns: Sequence[Pattern]) -> Pna:
+    """compile_positions for pattern sets it refuses: countable repeats (`C{lo,hi}`, one character leaf C, finite hi) become
+    lo expanded copies and one counter position each, the largest hi - lo first, until the automaton fits.  Within the
+    repeat the expanded NFA holds one count per entry since C's current run began; all grow by one per character and the
+    successors only need one in [1, k], so the newest entry's age is exact.  Raises PatternTooLarge when no number of
+    counters (at most PNA_MAX_COUNTERS) makes it fit."""
+    if len(patterns) > 32:
+        raise ValueError("at most 32 patterns per automaton")
+    cands = []                                        # (k, pattern, index into its _countable_repeats)
+    for pid, p in enumerate(patterns):
+        if p.kind == "regex":
+            ast = _P.parse(p.text, p.flags)
+            cands += [(k, pid, i) for i, (_node, k) in enumerate(_countable_repeats(ast.data, ast.state.flags, []))]
+    cands.sort(key=lambda c: (-c[0], c[1], c[2]))
+    why = "no repeat a counter can hold"
+    for m in range(1, len(cands) + 1):
+        chosen: Dict[int, List[int]] = {}
+        for _k, pid, i in cands[:m]:
+            chosen.setdefault(pid, []).append(i)
+        n = Nfa()
+        try:
+            for pid, p in enumerate(patterns):
+                add_pattern(n, pid, p, counted=chosen.get(pid, ()))
+            n.add_trailing_newline_rule()
+            return _pna_of(n, len(patterns))
+        except PatternTooLarge as e:
+            why = str(e)
+    raise PatternTooLarge(f"position automaton with counters: {why}")
+
+
+def _pna_of(n: Nfa, n_patterns: int) -> Pna:
     pos = _positions(n)
     n_pos = len(pos) + 1
     if n_pos > PNA_MAX_POS:
         raise PatternTooLarge(f"position automaton needs {n_pos} bits (limit {PNA_MAX_POS})")
+    counters = [(i + 1, n.bound[e]) for i, e in enumerate(pos) if e in n.bound]
+    if len(counters) > PNA_MAX_COUNTERS:
+        raise PatternTooLarge(f"position automaton needs {len(counters)} counters (limit {PNA_MAX_COUNTERS})")
+    counter_pos = {p for p, _k in counters}
     # code point classes: the leaves of the positions, plus the sets that decide a class' context kind
     uses = n.uses
     need_nl = A_BOL in uses or A_EOL in uses or A_NEXTNL in uses
@@ -1138,7 +1248,7 @@ def compile_positions(patterns: Sequence[Pattern]) -> Pna:
         for j, m in fm.items():
             if m == CTX_ALL and j == i + 1:
                 shift |= 1 << j
-            elif m == CTX_ALL and j == i:
+            elif m == CTX_ALL and j == i and j not in counter_pos:   # re-entering a counter is a fresh entry: a follow group
                 self_loop |= 1 << j
             else:
                 by_mask[m] = by_mask.get(m, 0) | (1 << j)
@@ -1153,7 +1263,7 @@ def compile_positions(patterns: Sequence[Pattern]) -> Pna:
     words = 1
     while words * 32 < n_pos:
         words *= 2
-    return Pna(n_words=words, n_pos=n_pos, n_patterns=len(patterns), ascii_cls=ascii_cls, ranges=ranges, cls_b=cls_b,
+    return Pna(n_words=words, n_pos=n_pos, n_patterns=n_patterns, ascii_cls=ascii_cls, ranges=ranges, cls_b=cls_b,
                cls_kind=kinds, shift=shift, self_loop=self_loop, start=1,
                follow=[(src, dst, m) for (dst, m), src in follow.items()],
-               accept=[(src, m, p, eo) for (m, p, eo), src in accept.items()])
+               accept=[(src, m, p, eo) for (m, p, eo), src in accept.items()], counters=counters)

@@ -245,6 +245,7 @@ typedef struct fei_scan_timing {
   uint32_t body_acc_mode;        /* how k_body records accepting states: 1 / 2 <= 32 / <= 64 of them as register bits,
                                     0 out[] per step, 3 single-pattern (sticky) automaton */
   uint32_t body_nfa_words;       /* k_body_nfa: 32-bit words per position vector (1, 2, 4 or 8); 0 for the other kernels */
+  uint32_t body_nfa_counters;    /* k_body_nfa: counter positions of the content automaton (feiscan_prog.h fei_prog_nfa_ctr), 0 = none */
 } fei_scan_timing;
 int fei_scan_last_timing(const fei_corpus* c, fei_scan_timing* out);
 

@@ -22,6 +22,8 @@
 #define FEI_PROG_VERSION_NFA 2u        /* written only by programs that carry at least one position automaton (fei_prog_nfa):
                                           content (off_body_nfa), a header slot (fei_prog_slot.off_val_nfa), flags or a name
                                           field (off_head_nfa) */
+#define FEI_PROG_VERSION_CTR 3u        /* written only by programs whose content position automaton has counters
+                                          (fei_prog_nfa_ctr); every other program keeps version 1 or 2 */
 #define FEI_MAX_QUERIES  32
 #define FEI_MAX_SLOTS    16
 
@@ -64,8 +66,9 @@ typedef struct fei_prog_hdr {            /* 96 bytes */
   uint32_t head_bytes;                   /* everything before the content automaton (which is serialised last): the part the
                                             head kernels copy into shared memory; 0 = unknown (do not stage)              */
   uint32_t off_meta_dfa[2];              /* name fields 3 and 4: automata over the formatted timestamp / date strings        */
-  uint32_t off_body_nfa;                 /* version 2 only: fei_prog_nfa of the content patterns too large for the body DFA; 0 = none */
-  uint32_t off_head_nfa;                 /* version 2 only: fei_prog_head_nfa (position automata of flags and the name fields); 0 = none */
+  uint32_t off_body_nfa;                 /* version 2 or 3: fei_prog_nfa of the content patterns too large for the body DFA; 0 = none
+                                            (version 3: present, with a fei_prog_nfa_ctr behind it) */
+  uint32_t off_head_nfa;                 /* version 2 or 3: fei_prog_head_nfa (position automata of flags and the name fields); 0 = none */
 } fei_prog_hdr;
 
 /* Position automaton (bit-parallel NFA, fei_b200/regexc compile_positions), for content patterns whose DFA is too
@@ -96,6 +99,20 @@ typedef struct fei_prog_nfa {            /* 64 bytes */
 #define FEI_NFA_MAX_CLASSES 128
 #define FEI_NFA_MAX_RANGES  4096
 #define FEI_NFA_MAX_GROUPS  64           /* follow groups, and accept groups, each */
+
+/* Counters of the content position automaton (fei_b200/regexc compile_positions_counted): in a version-3 program, and only
+ * there, this descriptor lies right behind the content fei_prog_nfa (at off_body_nfa + 64, before its tables); head fields
+ * never have one.  Counter position P with bound k stands for a whole repeat `C{1,k}` of one character class: besides the
+ * follow step, P stays set while C keeps matching and fewer than k code points have passed since its newest entry:
+ *     entered = F[P];  D'[P] = B[class(c)][P] && (entered || (D[P] && age_P < k));  age_P = entered ? 1 : age_P + 1
+ * with F = Follow(D, ctx) as above (every other bit is F & B[class(c)]); ages start at 0.  P is never in SELF and never
+ * the start bit. */
+typedef struct fei_prog_nfa_ctr {        /* 16 bytes */
+  uint32_t n_counters;                   /* 1 .. FEI_NFA_MAX_COUNTERS                                                         */
+  uint32_t off_counters;                 /* uint32[n_counters][2]: position, bound k >= 1; inside the section's tables        */
+  uint32_t reserved[2];
+} fei_prog_nfa_ctr;
+#define FEI_NFA_MAX_COUNTERS 8
 
 /* Position automata of flags and the name fields (fei_prog_hdr.off_head_nfa, inside [0, head_bytes)).  0 = the field has none;
  * a field with an automaton and no DFA has off_flags_dfa / off_name_dfa / off_meta_dfa 0. */
@@ -149,7 +166,7 @@ typedef struct fei_prog_slot {           /* 16 bytes */
                                                substring search); the key pattern of such a slot matches every key                      */
   uint32_t off_val_dfa;                  /* 0 = the slot has only a position automaton                                                   */
   uint32_t empty_if_missing;             /* 1: an absent header reads as "" (headers.get("Status", ""), search.py:118)                   */
-  uint32_t off_val_nfa;                  /* version 2 only: fei_prog_nfa of the slot's patterns its DFA cannot hold; 0 = none; at least
+  uint32_t off_val_nfa;                  /* version 2 or 3: fei_prog_nfa of the slot's patterns its DFA cannot hold; 0 = none; at least
                                             one of off_val_dfa / off_val_nfa is set                                                     */
 } fei_prog_slot;
 

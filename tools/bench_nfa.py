@@ -4,11 +4,12 @@
     tools/bench_nfa.py [--entries 10000000] [--steps 10] [--warmup 3] [--sample 20000]
 
 Workloads, each one program over the whole corpus: `kubernetes.*docker` (a DFA), three proximity patterns the DFA refuses
-(position vectors of 4 and 8 words), the first 31 patterns of the 32-pattern bench batch plus one proximity pattern (the
+(position vectors of 4 and 8 words), the longest gap the plain position automaton holds (`kubernetes.{0,238}docker`, 8 words)
+and three it refuses, which run with one counter (`{0,239}`, `{0,1000}`, `{0,5000}`), the first 31 patterns of the 32-pattern bench batch plus one proximity pattern (the
 DFA and the position automaton in one kernel) and the plain 32-pattern batch.  After a warm-up of every workload, the steps
 alternate the workloads; each step is one scan_count call, and the median body_ms / total_ms of the steps is reported with
-the content GB/s (body bytes of the corpus over body_ms), the kernel the scan ran (fei_scan_timing.body_kernel) and the
-words per position vector.  The hit counts are checked against CPython re on the first `--sample` records, fetched back from
+the content GB/s (body bytes of the corpus over body_ms), the kernel the scan ran (fei_scan_timing.body_kernel), the
+words per position vector and its counters.  The hit counts are checked against CPython re on the first `--sample` records, fetched back from
 the device.  The card's name and power limit are printed with the numbers.  Exits non-zero without a GPU."""
 import argparse, json, os, re, statistics, subprocess, sys
 
@@ -19,6 +20,7 @@ os.environ.setdefault("TZ", "UTC")
 import numpy as np  # noqa: E402
 
 PROXIMITY = [r"kubernetes.{0,60}docker", r"kubernetes.{0,200}docker", r"\bpython\b.{0,60}\b(rust|django)\b"]
+LONG_GAPS = [r"kubernetes.{0,238}docker", r"kubernetes.{0,239}docker", r"kubernetes.{0,1000}docker", r"kubernetes.{0,5000}docker"]
 
 
 def main():
@@ -41,7 +43,7 @@ def main():
     _abi.init(0)
     rx = lambda p: Pattern("regex", p, re.IGNORECASE)                     # noqa: E731
     work = {"dfa kubernetes.*docker": [r"kubernetes.*docker"]}
-    for p in PROXIMITY:
+    for p in PROXIMITY + LONG_GAPS:
         work["nfa " + p] = [p]
     work["batch31 + " + PROXIMITY[0]] = bench.BATCH32[:31] + [PROXIMITY[0]]
     work["batch32"] = list(bench.BATCH32)
@@ -74,6 +76,7 @@ def main():
         body_ms = statistics.median(t["body_ms"] for t in tms)
         row = {"workload": k, "body_ms": round(body_ms, 3), "total_ms": round(statistics.median(t["total_ms"] for t in tms), 3),
                "body_kernel": int(tms[-1]["body_kernel"]), "body_nfa_words": int(tms[-1]["body_nfa_words"]),
+               "body_nfa_counters": int(tms[-1]["body_nfa_counters"]),
                "body_GB_per_s": round(body_bytes / body_ms / 1e6, 1),
                "hits": int(np.sum(counts[k])), "sample_equals_re": sample_ok[k]}
         out.append(row)
