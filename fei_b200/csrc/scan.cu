@@ -1749,20 +1749,16 @@ __global__ void __launch_bounds__(NfaThreads<W, kCtr>::value, 1) k_body_nfa(Body
 }
 
 using BodyKernel = void (*)(BodyArgs);
-template <bool kCtr> static BodyKernel body_nfa_kernel(uint32_t words, bool has_dfa) {
-  switch (words) {
-    case 1: return has_dfa ? k_body_nfa<1, true, kCtr> : k_body_nfa<1, false, kCtr>;
-    case 2: return has_dfa ? k_body_nfa<2, true, kCtr> : k_body_nfa<2, false, kCtr>;
-    case 4: return has_dfa ? k_body_nfa<4, true, kCtr> : k_body_nfa<4, false, kCtr>;
-    default: return has_dfa ? k_body_nfa<8, true, kCtr> : k_body_nfa<8, false, kCtr>;
-  }
-}
-static BodyKernel body_nfa_kernel(uint32_t words, bool has_dfa, bool counters) {
-  return counters ? body_nfa_kernel<true>(words, has_dfa) : body_nfa_kernel<false>(words, has_dfa);
-}
-static int body_nfa_threads(uint32_t words, bool counters) {
-  if (counters) return words == 8 ? NfaThreads<8, true>::value : NfaThreads<4, true>::value;
-  return words == 8 ? NfaThreads<8>::value : NfaThreads<4>::value;
+// The k_body_nfa instance for a content automaton of `words` words (check_prog: 1, 2, 4 or 8) and its block size.
+struct BodyNfaKernel { BodyKernel k; int threads; };
+template <int W, bool kHasDfa, bool kCtr> constexpr BodyNfaKernel body_nfa_of() { return {k_body_nfa<W, kHasDfa, kCtr>, NfaThreads<W, kCtr>::value}; }
+static BodyNfaKernel body_nfa_kernel(uint32_t words, bool has_dfa, bool counters) {
+  static const BodyNfaKernel of[2][2][4] = {          // [counters][has_dfa][log2 words]
+      {{body_nfa_of<1, false, false>(), body_nfa_of<2, false, false>(), body_nfa_of<4, false, false>(), body_nfa_of<8, false, false>()},
+       {body_nfa_of<1, true, false>(), body_nfa_of<2, true, false>(), body_nfa_of<4, true, false>(), body_nfa_of<8, true, false>()}},
+      {{body_nfa_of<1, false, true>(), body_nfa_of<2, false, true>(), body_nfa_of<4, false, true>(), body_nfa_of<8, false, true>()},
+       {body_nfa_of<1, true, true>(), body_nfa_of<2, true, true>(), body_nfa_of<4, true, true>(), body_nfa_of<8, true, true>()}}};
+  return of[counters][has_dfa][__builtin_ctz(words)];
 }
 
 // The content kernel of one scan: k_body_sticky when the sticky automaton's row addresses fit 16 bits, else the k_body
@@ -1778,14 +1774,9 @@ static BodyKernel body_kernel(bool sticky, bool direct, int acc_mode, bool push)
 }
 
 template <typename Kernel, typename... Args>
-static int launch_body(Kernel k, unsigned grid, size_t smem, cudaStream_t s, Args... args) {
+static int launch_body(Kernel k, int threads, unsigned grid, size_t smem, cudaStream_t s, Args... args) {
   FEI_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  k<<<grid, kBodyThreads, smem, s>>>(args...);
-  return FEI_OK;
-}
-static int launch_body_nfa(BodyKernel k, int threads, unsigned grid, size_t smem, cudaStream_t s, BodyArgs a) {
-  FEI_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  k<<<grid, threads, smem, s>>>(a);
+  k<<<grid, threads, smem, s>>>(args...);
   return FEI_OK;
 }
 
@@ -1933,9 +1924,11 @@ static int check_prog(const uint8_t* prog, uint64_t len) {
   if (!dfa_ok(h.off_key_dfa) || !dfa_ok(h.off_body_dfa) || !dfa_ok(h.off_flags_dfa) || !dfa_ok(h.off_name_dfa[0]) ||
       !dfa_ok(h.off_name_dfa[1]) || !dfa_ok(h.off_name_dfa[2]) || !dfa_ok(h.off_meta_dfa[0]) || !dfa_ok(h.off_meta_dfa[1])) { set_error("bad DFA descriptor in program"); return FEI_E_BADARG; }
   // A position automaton section (0 = none): every table inside its table_bytes; a head one inside [0, head_bytes) when the head
-  // kernels stage the head.
+  // kernels stage the head.  Counters: version 3 if and only if the content automaton has a fei_prog_nfa_ctr right behind its
+  // descriptor (the head ones never have one), with its table among the section's; ctr_ok says whether it is well-formed.
   uint32_t n_nfa = 0;
-  auto nfa_ok = [&](uint32_t off, bool head) {
+  bool ctr_ok = h.version != FEI_PROG_VERSION_CTR;
+  auto nfa_ok = [&](uint32_t off, bool content) {
     if (!off) return true;
     ++n_nfa;
     if (!in(off, sizeof(fei_prog_nfa))) return false;
@@ -1948,7 +1941,7 @@ static int check_prog(const uint8_t* prog, uint64_t len) {
               a.table_bytes % 16 == 0 && in(a.off_ascii, a.table_bytes) && tab(a.off_ascii, 2 * 128) &&
               tab(a.off_range_lo, 4ull * a.n_ranges) && tab(a.off_range_ck, 2ull * a.n_ranges) && tab(a.off_cls_b, 4ull * W * a.n_classes) &&
               tab(a.off_masks, 12ull * W) && tab(a.off_follow, 4ull * (2 * W + 1) * a.n_follow) && tab(a.off_accept, 4ull * (W + 2) * a.n_accept) &&
-              (!head || !h.head_bytes || (off + sizeof(fei_prog_nfa) <= h.head_bytes && end <= h.head_bytes));
+              (content || !h.head_bytes || (off + sizeof(fei_prog_nfa) <= h.head_bytes && end <= h.head_bytes));
     if (ok) {                                      // class ids index cls_b, kinds are 0..4, the range table starts at 0x80
       const uint16_t* asc = reinterpret_cast<const uint16_t*>(prog + a.off_ascii);
       const uint16_t* rck = reinterpret_cast<const uint16_t*>(prog + a.off_range_ck);
@@ -1959,41 +1952,36 @@ static int check_prog(const uint8_t* prog, uint64_t len) {
       const uint32_t* acc = reinterpret_cast<const uint32_t*>(prog + a.off_accept);
       for (uint32_t g = 0; g < a.n_accept && ok; ++g) ok = (acc[g * (W + 2) + W + 1] & 0xFFu) < 32;
     }
+    if (ok && content && h.version == FEI_PROG_VERSION_CTR) {
+      fei_prog_nfa_ctr cd{};
+      const uint64_t at = (uint64_t)off + sizeof(a);
+      ctr_ok = in(at, sizeof(cd)) && a.off_ascii >= at + sizeof(cd);
+      if (ctr_ok) memcpy(&cd, prog + at, sizeof(cd));
+      ctr_ok = ctr_ok && cd.n_counters >= 1 && cd.n_counters <= FEI_NFA_MAX_COUNTERS && tab(cd.off_counters, 8ull * cd.n_counters);
+      const uint32_t* ct = reinterpret_cast<const uint32_t*>(prog + cd.off_counters);
+      const uint32_t* self_loop = reinterpret_cast<const uint32_t*>(prog + a.off_masks) + W;
+      for (uint32_t i = 0; i < cd.n_counters && ctr_ok; ++i) {
+        const uint32_t pos = ct[2 * i], bound = ct[2 * i + 1];
+        ctr_ok = pos >= 1 && pos < a.n_pos && !(self_loop[pos >> 5] >> (pos & 31u) & 1u) && bound >= 1;
+      }
+    }
     return ok;
   };
   const fei_prog_slot* sl = reinterpret_cast<const fei_prog_slot*>(prog + h.off_slots);
   for (uint32_t s = 0; s < h.n_slots; ++s)
-    if ((!sl[s].off_val_dfa && !sl[s].off_val_nfa) || !dfa_ok(sl[s].off_val_dfa) || !nfa_ok(sl[s].off_val_nfa, true)) { set_error("bad slot automaton"); return FEI_E_BADARG; }
+    if ((!sl[s].off_val_dfa && !sl[s].off_val_nfa) || !dfa_ok(sl[s].off_val_dfa) || !nfa_ok(sl[s].off_val_nfa, false)) { set_error("bad slot automaton"); return FEI_E_BADARG; }
   if (h.n_slots && !h.off_key_dfa) { set_error("slots without a key DFA"); return FEI_E_BADARG; }
   if (h.off_head_nfa) {                            // flags and name fields
     fei_prog_head_nfa hn;
     if (!in(h.off_head_nfa, sizeof(hn)) || (h.head_bytes && h.off_head_nfa + sizeof(hn) > h.head_bytes)) { set_error("head position automata out of bounds"); return FEI_E_BADARG; }
     memcpy(&hn, prog + h.off_head_nfa, sizeof(hn));
-    bool ok = nfa_ok(hn.off_flags_nfa, true);
-    for (int k = 0; k < FEI_NAME_FIELDS && ok; ++k) ok = nfa_ok(hn.off_name_nfa[k], true);
+    bool ok = nfa_ok(hn.off_flags_nfa, false);
+    for (int k = 0; k < FEI_NAME_FIELDS && ok; ++k) ok = nfa_ok(hn.off_name_nfa[k], false);
     if (!ok) { set_error("bad flags / name position automaton in program"); return FEI_E_BADARG; }
   }
-  if (!nfa_ok(h.off_body_nfa, false)) { set_error("bad content position automaton in program"); return FEI_E_BADARG; }
+  if (!nfa_ok(h.off_body_nfa, true)) { set_error("bad content position automaton in program"); return FEI_E_BADARG; }
   if ((h.version != FEI_PROG_VERSION) != (n_nfa != 0)) { set_error("bad program magic/version"); return FEI_E_BADARG; }
-  // counters: version 3 if and only if the content automaton has a fei_prog_nfa_ctr (the head ones never have one)
-  if (h.version == FEI_PROG_VERSION_CTR) {
-    fei_prog_nfa a; fei_prog_nfa_ctr cd;
-    const uint64_t at = (uint64_t)h.off_body_nfa + sizeof(a);
-    bool ok = h.off_body_nfa != 0 && in(at, sizeof(cd));
-    if (ok) {
-      memcpy(&a, prog + h.off_body_nfa, sizeof(a)); memcpy(&cd, prog + at, sizeof(cd));
-      const uint64_t W = a.n_words, end = (uint64_t)a.off_ascii + a.table_bytes;
-      ok = a.off_ascii >= at + sizeof(cd) && cd.n_counters >= 1 && cd.n_counters <= FEI_NFA_MAX_COUNTERS &&
-           cd.off_counters % 16 == 0 && cd.off_counters >= a.off_ascii && cd.off_counters + 8ull * cd.n_counters <= end;
-      const uint32_t* tab = reinterpret_cast<const uint32_t*>(prog + cd.off_counters);
-      const uint32_t* self_loop = reinterpret_cast<const uint32_t*>(prog + a.off_masks) + W;
-      for (uint32_t i = 0; i < cd.n_counters && ok; ++i) {
-        const uint32_t pos = tab[2 * i], bound = tab[2 * i + 1];
-        ok = pos >= 1 && pos < a.n_pos && !(self_loop[pos >> 5] >> (pos & 31u) & 1u) && bound >= 1;
-      }
-    }
-    if (!ok) { set_error("bad counters of the content position automaton in program"); return FEI_E_BADARG; }
-  }
+  if (!ctr_ok) { set_error("bad counters of the content position automaton in program"); return FEI_E_BADARG; }
   if (h.off_body_nfa) {
     fei_prog_dfa d{};
     if (h.off_body_dfa) memcpy(&d, prog + h.off_body_dfa, sizeof(d));
@@ -2175,7 +2163,7 @@ int run_scan(fei_corpus* c, const uint8_t* prog, uint64_t prog_len, int compact_
     a.gather_max = n / kGatherDiv;
     FEI_TRY(c->live_list.ensure((a.gather_max + 1) * sizeof(uint32_t)));
     k_live_list<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(c->hits.as<uint32_t>(), n, c->live_list.as<uint32_t>(), a.counter + 4, a.gather_max);
-    FEI_TRY(launch_body(k_body_gather, grid, smem, s, a, c->live_list.as<uint32_t>(), c->rec_pos.as<uint32_t>()));
+    FEI_TRY(launch_body(k_body_gather, kBodyThreads, grid, smem, s, a, c->live_list.as<uint32_t>(), c->rec_pos.as<uint32_t>()));
     launches += 2;
   }
   if (body_lists || push) {                                    // window counters (and, for body_lists, descriptors) for the scan
@@ -2192,12 +2180,12 @@ int run_scan(fei_corpus* c, const uint8_t* prog, uint64_t prog_len, int compact_
   }
   if (push) { a.push_peers = hook->push_peers; a.push_n = hook->push_n; a.push_off = hook->push_off; hook->pushed = true; }
   if (n && nfa) {
-    const bool counters = c->timing.body_nfa_counters != 0;
-    FEI_TRY(launch_body_nfa(body_nfa_kernel(na.n_words, h.off_body_dfa != 0, counters), body_nfa_threads(na.n_words, counters), grid, smem, s, a));
+    const BodyNfaKernel k = body_nfa_kernel(na.n_words, h.off_body_dfa != 0, c->timing.body_nfa_counters != 0);
+    FEI_TRY(launch_body(k.k, k.threads, grid, smem, s, a));
     ++launches;
   } else if (n && need_body) {
     const size_t body_smem = sticky_kernel ? ((smem + 127) & ~(size_t)127) + kStickyRingBytes : smem;   // k_body_sticky: + its rings
-    FEI_TRY(launch_body(body_kernel(sticky_kernel, direct, acc_mode, a.push_n != 0), grid, body_smem, s, a));
+    FEI_TRY(launch_body(body_kernel(sticky_kernel, direct, acc_mode, a.push_n != 0), kBodyThreads, grid, body_smem, s, a));
     ++launches;
   }
   FEI_CUDA(cudaEventRecord(c->ev[3], s));

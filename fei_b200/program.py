@@ -57,7 +57,6 @@ def _pad16(b: bytearray) -> None:
 _DFA_CACHE: Dict[Tuple, Dfa] = {}
 _DFA_FAIL: Dict[Tuple, str] = {}       # same keys: pattern sets whose DFA was refused (PatternTooLarge), with the reason
 _PNA_CACHE: Dict[Tuple, Pna] = {}
-_PNA_CTR_CACHE: Dict[Tuple, Pna] = {}
 
 
 def _remember(cache: Dict, key, value) -> None:
@@ -90,32 +89,20 @@ def cached_dfa(patterns: Sequence[Pattern], sticky: bool = False) -> Dfa:
     return d
 
 
-def cached_positions(patterns: Sequence[Pattern]) -> Pna:
-    key = tuple(_pkey(p) for p in patterns)
+def cached_positions(patterns: Sequence[Pattern], counters: bool = False) -> Pna:
+    """The position automaton of `patterns`, cached per process.  With `counters` (content), compile_positions_counted where
+    the plain automaton is refused (long bounded gaps such as `a.{0,1000}b`); head fields keep the plain one."""
+    key = (tuple(_pkey(p) for p in patterns), counters)
     a = _PNA_CACHE.get(key)
     if a is None:
-        a = compile_positions(patterns)
+        try:
+            a = compile_positions(patterns)
+        except PatternTooLarge:
+            if not counters:
+                raise
+            a = compile_positions_counted(patterns)
         _remember(_PNA_CACHE, key, a)
     return a
-
-
-def cached_counted_positions(patterns: Sequence[Pattern]) -> Pna:
-    """compile_positions_counted, cached per process like cached_positions."""
-    key = tuple(_pkey(p) for p in patterns)
-    a = _PNA_CTR_CACHE.get(key)
-    if a is None:
-        a = compile_positions_counted(patterns)
-        _remember(_PNA_CTR_CACHE, key, a)
-    return a
-
-
-def content_positions(patterns: Sequence[Pattern]) -> Pna:
-    """The position automaton of content patterns: the plain one, or the one with counters where the plain one is refused
-    (long bounded gaps such as `a.{0,1000}b`)."""
-    try:
-        return cached_positions(patterns)
-    except PatternTooLarge:
-        return cached_counted_positions(patterns)
 
 
 def content_automaton(p: Pattern):
@@ -125,7 +112,7 @@ def content_automaton(p: Pattern):
     try:
         return cached_dfa([p])
     except PatternTooLarge:
-        return content_positions([p])
+        return cached_positions([p], counters=True)
 
 
 class _FieldDfa:
@@ -259,18 +246,17 @@ def serialize_nfa(a: Pna, blob: bytearray, first_bit: int) -> int:
     return desc_off
 
 
-def _route(patterns: Sequence[Pattern], fits, sticky: bool = False) -> Tuple[List[int], List[int], Optional[Pna]]:
+def _route(patterns: Sequence[Pattern], fits, content: bool = False) -> Tuple[List[int], List[int], Optional[Pna]]:
     """Which of one field's patterns its DFA takes and which go to the position automaton: (dfa indices, nfa indices, the
     automaton of the nfa ones).  The union goes to the DFA whenever it compiles and fits, exactly as without the position
     automaton.  Otherwise every pattern whose DFA is refused (or does not fit) on its own goes to the position automaton, and
     then the patterns with the largest DFAs until the union of the rest fits.  The field's size rule is
-    fits(dfa, pna, whole): whether `dfa` fits next to position automaton `pna` (None: alone); `whole` marks the first try,
-    the union compiled with `sticky`.  Content (fits is _body_fits) takes the automaton with counters where the plain one is
-    refused; head fields keep the plain one."""
-    positions = content_positions if fits is _body_fits else cached_positions
+    fits(dfa, pna, whole): whether `dfa` fits next to position automaton `pna` (None: alone); `whole` marks the first try.
+    `content` selects the body kernel's rules: the union compiled sticky, and the position automaton with counters where the
+    plain one is refused (cached_positions(..., counters=True)); head fields keep a plain union and the plain automaton."""
     idx = list(range(len(patterns)))
     try:
-        if fits(cached_dfa(patterns, sticky=sticky), None, True):
+        if fits(cached_dfa(patterns, sticky=content), None, True):
             return idx, [], None
     except PatternTooLarge:
         pass
@@ -285,7 +271,7 @@ def _route(patterns: Sequence[Pattern], fits, sticky: bool = False) -> Tuple[Lis
     dfa = [i for i in idx if i in size]
     while True:
         nfa = [i for i in idx if i not in dfa]
-        a = positions([patterns[i] for i in nfa])
+        a = cached_positions([patterns[i] for i in nfa], counters=content)
         if not dfa:
             break
         try:
@@ -310,7 +296,7 @@ def _head_fits(d: Dfa, a: Optional[Pna], whole: bool) -> bool:
 
 
 def _route_body(patterns: Sequence[Pattern]) -> Tuple[List[int], List[int], Optional[Pna]]:
-    return _route(patterns, _body_fits, sticky=True)
+    return _route(patterns, _body_fits, True)
 
 
 def _nfa_table_bytes(a: Pna) -> int:

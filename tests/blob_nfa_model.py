@@ -1,19 +1,22 @@
 """CPU model of a serialized content position automaton (fei_b200/program.py serialize_nfa, include/feiscan_prog.h
 fei_prog_nfa): reads the section out of a program blob and steps a stored body the way k_body_nfa does -- undo the tile byte
 permutation, decode UTF-8, look the class up (ASCII table, else a binary search over the range table), step the W-word
-vector -- next to the program's body DFA when it has one, so a test can tell a wrong table from a wrong kernel."""
+vector -- next to the program's body DFA when it has one, so a test can tell a wrong table from a wrong kernel.  The content
+section of a version-3 program also has counter positions (fei_prog_nfa_ctr right behind the descriptor), stepped the way
+k_body_nfa's counted instances do -- per counter position P with bound k,
+    entered = F[P];  D'[P] = B[class][P] && (entered || (D[P] && age_P < k));  age_P = entered ? 1 : age_P + 1"""
 import struct
 
 import numpy as np
 
-from fei_b200.program import tile_byte_perm
+from fei_b200.program import VERSION_CTR, tile_byte_perm
 from tests.blob_model import BlobDfa
 
 _TILE_BYTE = tile_byte_perm(np.arange(256)).tolist()
 
 
 class BlobNfa:
-    def __init__(self, blob: bytes, off: int):
+    def __init__(self, blob: bytes, off: int, counters: bool = False):
         (self.W, self.n_pos, self.n_classes, self.n_ranges, self.n_follow, self.n_accept, self.n_patterns, self.first_bit,
          off_ascii, off_lo, off_rck, off_b, off_masks, off_follow, off_accept, self.table_bytes) = struct.unpack_from("<16I", blob, off)
         W = self.W
@@ -33,10 +36,16 @@ class BlobNfa:
         self.follow = [(vec(r[:W]), vec(r[W:2 * W]), r[2 * W]) for r in (f[g * (2 * W + 1):(g + 1) * (2 * W + 1)] for g in range(self.n_follow))]
         a = u32(off_accept, self.n_accept * (W + 2))
         self.accept = [(vec(r[:W]), r[W], r[W + 1] & 0xFF, bool(r[W + 1] >> 8)) for r in (a[g * (W + 2):(g + 1) * (W + 2)] for g in range(self.n_accept))]
+        self.counters = []                                                # (position, bound) of each counter position
+        if counters:
+            n, off_ctr = struct.unpack_from("<2I", blob, off + 64)                 # fei_prog_nfa_ctr
+            tab = struct.unpack_from(f"<{2 * n}I", blob, off_ctr)
+            self.counters = [(tab[2 * i], tab[2 * i + 1]) for i in range(n)]
 
     @classmethod
     def from_program(cls, prog: bytes) -> "BlobNfa":
-        return cls(prog, struct.unpack_from("<I", prog, 88)[0])           # fei_prog_hdr.off_body_nfa
+        """The content section (fei_prog_hdr.off_body_nfa), with its counters when the program is version 3."""
+        return cls(prog, struct.unpack_from("<I", prog, 88)[0], struct.unpack_from("<I", prog, 4)[0] == VERSION_CTR)
 
     def class_kind(self, cp: int) -> int:
         if cp < 0x80:
@@ -62,6 +71,7 @@ class BlobNfa:
         as the kernel reads it."""
         d, prev, acc = self.start, 0, 0
         cp, need = 0, 0
+        age = [0] * len(self.counters)
         for raw in body:
             byte = _TILE_BYTE[_TILE_BYTE[raw]]
             if byte < 0x80:
@@ -83,7 +93,12 @@ class BlobNfa:
             for src, dst, m in self.follow:
                 if m & ctx and d & src:
                     nd |= dst
-            d = nd & self.cls_b[c]
+            keep = 0
+            for i, (p, k) in enumerate(self.counters):
+                if d >> p & 1 and age[i] < k:
+                    keep |= 1 << p
+                age[i] = 1 if nd >> p & 1 else age[i] + 1
+            d = (nd | keep) & self.cls_b[c]
             prev = kind
         return acc | self._accepts(d, 1 << (prev * 5), True)
 

@@ -1,6 +1,6 @@
 """Position automata with counters (CPU suite): fei_b200.regexc.compile_positions_counted against CPython's
 re.search(p, s, re.I) on fixed cases and a seeded fuzz (bounds from 239 to 100000, the usual gap classes, lower bounds, lazy
-repeats, anchors next to the gap, nested and several patterns), the serialized counter section (tests/blob_nfa_ctr_model.py)
+repeats, anchors next to the gap, nested and several patterns), the serialized counter section (tests/blob_nfa_model.py)
 against Pna.run, the refusals, and the routing: only content patterns the plain automaton refuses get counters and a version-3
 program; head fields keep their limits."""
 import random
@@ -12,7 +12,7 @@ import pytest
 from fei_b200.program import (C_BODY, C_SLOT, VERSION_CTR, VERSION_NFA, Cond, ProgramBuilder, _route_body, content_automaton,
                               content_batch_program)
 from fei_b200.regexc import PNA_MAX_COUNTERS, Pattern, PatternTooLarge, compile_positions, compile_positions_counted
-from tests.blob_nfa_ctr_model import BlobNfaCtr, program_content_bits
+from tests.blob_nfa_model import BlobNfa, program_content_bits
 
 BOUNDS = [239, 300, 1000, 5000, 100000]
 CLASSES = [".", "(?s:.)", r"[\s\S]", r"[^\n]", r"\W", "[^x]", r"\w"]
@@ -122,7 +122,7 @@ def test_serialized_counters_agree_with_the_automaton():
     for pats in ([r"kubernetes.{0,1000}docker"], [r"q\W{0,300}z", "plain"], [r"docker", r"(?:a.{0,300}b){2}", r"q.{0,60}z"]):
         prog = content_batch_program([_rx(p) for p in pats])
         assert struct.unpack_from("<I", prog, 4)[0] == VERSION_CTR
-        m = BlobNfaCtr.from_program(prog)
+        m = BlobNfa.from_program(prog)
         assert m.counters
         dfa, nfa, _a = _route_body([_rx(p) for p in pats])
         bit = {i: b for b, i in enumerate(dfa + nfa)}                           # content bits: the DFA's first
